@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""GRPO-step throughput of the B200-native BioReason hot path (BASELINE.json metric), plus the CPU reference arm.
+"""GRPO-step throughput of the BioReason CUDA hot path (BASELINE.json metric), plus the CPU reference arm.
 
   python bench.py --gpus N --steps K --warmup W            # our arm (torchrun launches N ranks for N > 1)
   python bench.py --impl reference --gpus N --steps K ...  # the reference's HF/PyTorch path on the host cores (oracle)
@@ -42,11 +42,39 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-sweep", action="store_true", help="skip the secondary resident-row lines (16 / 32 rows per GPU)")
     ap.add_argument("--cpu-budget-s", type=float, default=25.0)
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed to DIR/<name>.npy (float32 / float64)")
+    args = ap.parse_args()
+    if args.dump_outputs and args.impl != "b200":
+        ap.error("--dump-outputs writes the arrays of the CUDA arm's timed step; the reference arm times a composed CPU sample")
+    return args
+
+
+def dump_outputs(trainer, loss, out_dir, max_sample=1 << 20):
+    """The arrays a caller of the timed step receives: the loss it returns, the rollout it buffered (completion ids, reference and
+    behaviour log-probs, advantages) and the LoRA gradient it accumulated (a fixed, seeded sample of at most `max_sample` entries)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    ga = trainer.args.gradient_accumulation_steps
+    inputs = trainer._buffered_inputs[(trainer._step - 1) % ga]
+    arrays = {"loss": loss.detach().reshape(1).double(), "completion_ids": inputs["completion_ids"].double(),
+              "advantages": inputs["advantages"].double()}
+    for name in ("ref_per_token_logps", "old_per_token_logps"):
+        if inputs.get(name) is not None:
+            arrays[name] = inputs[name].float()
+    g = trainer.model._lora.flat_grad.detach().float().reshape(-1)
+    if g.numel() > max_sample:
+        idx = torch.randperm(g.numel(), generator=torch.Generator().manual_seed(0))[:max_sample].sort().values
+        arrays["lora_grad_sample_index"] = idx.double()
+        g = g[idx.to(g.device)]
+    arrays["lora_grad"] = g
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy())
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# clocks sampling during the timed region (B200_PROFILING.md)
+# clocks sampling during the timed region
 # ----------------------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
@@ -211,14 +239,19 @@ def run_b200(args):
 
     loss_host = torch.zeros(1).pin_memory()
 
+    last = [None]
+
     def e2e_step():
         loss = trainer.training_step(to_device())                        # H2D of this step's inputs from pinned memory
         loss_host.copy_(loss.detach().reshape(1), non_blocking=False)    # D2H read of the step's result
+        last[0] = loss
     ms_e2e = timed(args.steps, e2e_step, tag="e2e")
     clk = clocks.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(trainer, last[0], args.dump_outputs)
 
     # ---- roofline of the dominant kernel: the decode weight-streaming GEMM, timed alone with CUDA events (weights of all
-    #      layers = 8 GB >> 126 MB L2, so every launch reads HBM)
+    #      layers = 8 GB >> 50 MB L2, so every launch reads HBM)
     work = algorithmic_work(tc, dc, args)
     W = model._rollout_dec or model._dec
     scratch = ops.skinny_scratch(max(tc.vocab_size, 2 * tc.intermediate_size), "cuda")
@@ -249,18 +282,14 @@ def run_b200(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = peaks.get("hbm_gbs", 6650.0)
-    tf_peak = peaks.get("bf16_tflops_sustained", 1400.0)
+    hbm_peak = peaks.get("hbm_gbs", 3350.0)                               # H100 SXM data sheet: 3.35 TB/s HBM3, 989 TFLOP/s dense BF16
+    tf_peak = peaks.get("bf16_tflops_sustained", 989.0)
     ach = bytes_k / (ms_k * 1e-3) / 1e9
     t_step = ms / args.steps / 1e3
     decode_s = gpu_phase.get("rollout", phase.get("rollout", 0.0))
     dense_s = max(t_step - decode_s, 1e-9)
     roofline = {"bound": "hbm", "kernel": "skinny_tc5_kernel (decode weight streaming, %d launches = all GEMMs of one token step for the group, CUDA-graph replay)" % n_k,
                 "achieved": round(ach, 1), "peak": hbm_peak, "unit": "GB/s", "frac": round(ach / hbm_peak, 4),
-                # dram__bytes_read+write per launch from the committed `ncu --set full` capture: 50.10 MB for the 49.81 MB down_proj launch and
-                # dram read+write 31.6 MB for the 31.46 MB qkv launch, 21.1 / 20.97 (o), 102.9 / 99.6 (gate/up incl. 3.2 MB written), 50.1 / 49.8
-                # (down): profiles/r02_ncu_targets.txt -> 1.005 .. 1.03 x the algorithmic bytes; the launch-weighted mean is used
-                "traffic": int(1.012 * bytes_k / n_k), "traffic_source": "ncu --set full capture, dram bytes / algorithmic bytes = 1.012 (profiles/r02_ncu_targets.txt)",
                 "peak_source": "MEASURED_PEAKS.json" if peaks else "fallback",
                 "bytes_per_launch_avg": int(bytes_k / n_k), "launch_us_avg": round(ms_k * 1e3 / n_k, 2),
                 "phases": {"rollout_s": round(decode_s, 4), "rollout_hbm_frac": round(work["decode_bytes"] / max(decode_s, 1e-9) / 1e9 / hbm_peak, 4),
@@ -278,8 +307,8 @@ def run_b200(args):
             "step_ms": per_step, "mem_gb": {"max_allocated": round(torch.cuda.max_memory_allocated() / 2 ** 30, 1),
                                             "max_reserved": round(torch.cuda.max_memory_reserved() / 2 ** 30, 1)}}
     # ---- secondary lines: more prompt groups resident per GPU (NOT the benchmark configuration: BASELINE config (c) is one group of
-    #      G = 8; the decode weight stream is amortised over more rows).  Row-chunked forward/backward (micro_rows = 8) keeps the
-    #      activation footprint of the 8-row step.
+    #      G = 8; the decode weight stream is amortised over more rows).  The forward/backward is row-chunked to what the device
+    #      memory holds.
     if world == 1 and not args.no_sweep and args.prompts_per_gpu == 1:
         import copy
         sweep = []
@@ -290,7 +319,7 @@ def run_b200(args):
                 a2 = copy.copy(args); a2.prompts_per_gpu = ppg
                 B2 = args.G * ppg
                 cfg2 = DNALLMGRPOConfig(num_generations=args.G, max_completion_length=args.completion, per_device_train_batch_size=B2,
-                                        suppress_eos=True, micro_rows=args.G, seed=1234)
+                                        suppress_eos=True, micro_rows=args.micro_rows or None, seed=1234)
                 tr2 = DNALLMGRPOTrainer(model, [synthetic_reward], cfg2)
                 hb = make_prompt_batch(tc, dc, a2, seed=1000 + rank)
                 res2 = dict(input_ids=hb["input_ids"].cuda(), attention_mask=hb["attention_mask"].cuda(),
@@ -298,7 +327,7 @@ def run_b200(args):
                 for _ in range(2):
                     tr2.training_step(res2)
                 ms2 = timed(2, lambda: tr2.training_step(res2)) / 2
-                sweep.append({"rows_per_gpu": B2, "prompts_per_gpu": ppg, "micro_rows": args.G, "value": round(B2 * args.completion / (ms2 / 1e3), 1),
+                sweep.append({"rows_per_gpu": B2, "prompts_per_gpu": ppg, "value": round(B2 * args.completion / (ms2 / 1e3), 1),
                               "ms_per_step": round(ms2, 1)})
                 del tr2, res2
                 torch.cuda.empty_cache()
@@ -449,7 +478,7 @@ def bench_config(args, world):
     """The `config` object both arms print (same keys, same values: the driver compares them)."""
     B = args.G * args.prompts_per_gpu
     return {"workload": workload_string(args), "shapes": f"{args.dna}+{args.text}", "rows_per_gpu": B, "parallelism": f"dp{world}",
-            "l2": "weights (8 GB) and activations (>60 GB) exceed the 126 MB L2 every step; no flush needed",
+            "l2": "weights (8 GB) and activations (>30 GB) exceed the 50 MB L2 every step; no flush needed",
             "weights": "seeded random init (no checkpoints offline)"}
 
 

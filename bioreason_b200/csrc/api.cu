@@ -27,7 +27,7 @@ int br_device_ok(void) {
     int dev = 0, major = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) { br_set_error("no CUDA device"); return 0; }
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-    if (major != 10) { br_set_error("libbioreason_b200 targets sm_100a only (found sm_%d)", major * 10); return 0; }
+    if (major != 9) { br_set_error("libbioreason_b200 targets sm_90a only (found sm_%d)", major * 10); return 0; }
     return 1;
 }
 

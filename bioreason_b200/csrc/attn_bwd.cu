@@ -1,5 +1,5 @@
 // C entry points of the flash-attention backward (br_attn_bwd, br_attn_bwd_workspace_bytes): argument checks + dispatch to the two
-// deterministic tcgen05 kernels in attn_bwd_tc5.cu.  (Round 1's mma.sync kernel with fp32 dQ atomics lived here; removed.)
+// deterministic wgmma kernels in attn_bwd_tc5.cu.
 #include "br_common.cuh"
 #include "../../include/bioreason_b200.h"
 

@@ -1,37 +1,30 @@
-// Flash attention backward on tcgen05 / TMEM / TMA (sm_100a; causal GQA decoder rows, head_dim 128) -- autograd counterpart of
+// Flash attention backward on wgmma / TMA (sm_90a; causal GQA decoder rows, head_dim 128) -- autograd counterpart of
 // attn_fwd_tc5.cu (SURVEY.md §2.3 K12).  Probabilities are recomputed from Q, K and the saved log-sum-exp; no score matrix, no
 // fp32 atomics and no dQ workspace ever touch HBM, and every output element is produced by exactly one CTA in a fixed order, so
 // the gradients are bit-reproducible run to run.
 //
-// Two kernels (7 tile GEMMs per (query tile, key tile) pair instead of the 5 of an atomics-based single pass; all on tcgen05):
-//   dq kernel   : CTA = 128-query tile of one (row, query head); loops over the 64-key tiles it can see.
-//                   S  = Q K^T              (SS: both operands K-major in shared memory, N = 64)
-//                   dP = dO V^T             (SS)
-//                   dS = P o (dP - delta) * scale   one thread per query row (TMEM lane), bf16 into TMEM over dP
-//                   dQ += dS K              (TS: A = dS in TENSOR MEMORY, B = the K tile as it landed, MN-major descriptor)
-//                 three score buffers (all 512 TMEM columns): S / dP of tile t + 2 are issued while tiles t, t + 1 are in the two groups;
+// Two kernels, one warpgroup per CTA, everything element-wise in registers (a quad of lanes shares a row of the tile):
+//   dq kernel   : CTA = 64-query tile of one (row, query head); loops over the 64-key tiles it can see.
+//                   S  = Q K^T,  dP = dO V^T                  (wgmma, both operands K-major in shared memory)
+//                   dS = P o (dP - delta) * scale
+//                   dQ += dS K                               (dS as the register A operand, the K tile as it landed, MN-major)
 //                 also computes delta = rowsum(dO o O) for its rows and publishes it for the dk/dv kernel.
-//   dk/dv kernel: CTA = 128-key tile of one (row, kv head); loops over the query heads of the group and the 64-query tiles that
-//                 can see the keys; dK and dV accumulate in TMEM for the whole loop.
-//                   S^T  = K Q^T,  dP^T = V dO^T                 (SS, N = 64)
-//                   P^T, dS^T (one thread per key row) bf16 into TMEM over S^T / dP^T
-//                   dV += P^T dO,  dK += dS^T Q                  (TS; dO and Q tiles are MN-major B operands)
-// Pipelining: S / dP (S^T / dP^T) are DOUBLE-BUFFERED in TMEM (4 x 64 columns) and two element-wise warpgroups alternate tiles, so the
-// tensor pipe computes the scores of tile t+1 while tile t is in its exp2 stage and the two groups sit in different phases of the
-// chain (scores ready -> tcgen05.ld -> exp2 -> tcgen05.st -> operand ready).  The first tcgen05 version used one score buffer and
-// 256 threads in lock-step on 128-wide tiles: tensor pipe idle during the whole element-wise stage, 30 % / 32 % active under ncu.
-// TMEM: 512 / 512 columns; one CTA per SM (~180 / 162 KB of shared memory: two resident tiles + 3- or 4-stage rings of the two streamed tiles).
+//   dk/dv kernel: CTA = 64-key tile of one (row, kv head); loops over the query heads of the group and the 64-query tiles that
+//                 can see the keys; dK and dV accumulate in registers for the whole loop.
+//                   S^T = K Q^T,  dP^T = V dO^T
+//                   dV += P^T dO,  dK += dS^T Q               (P^T / dS^T as register A operands; dO and Q tiles MN-major)
+// Thread 0 streams the per-iteration tiles through a two-stage TMA ring.
 #include "br_common.cuh"
 #include "../../include/bioreason_b200.h"
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int D = 128, BT = 128, BS = 64, NTHREADS = 320;   // warp 0 TMA, warp 1 MMA, warps 2..5 / 6..9 element-wise groups 0 / 1
-constexpr int BLK = BT * 128;             // bytes of a [128 rows x 64 cols] swizzled block (resident tiles)
-constexpr int BLKS = BS * 128;            // bytes of a [64 rows x 64 cols] swizzled block (streamed tiles)
-constexpr int TILE = 2 * BLK;             // a 128 x 128 bf16 tile
-constexpr int TILES = 2 * BLKS;           // a 64 x 128 bf16 tile
-constexpr int NST = 3;                    // ring depth of the streamed tiles
+constexpr int D = 128, BT = 64, NTHREADS = 128;
+constexpr int BLK = 64 * 128;             // bytes of a [64 rows x 64 cols] swizzled block
+constexpr int TILE = 2 * BLK;             // a 64 x 128 bf16 tile
+constexpr int OFF_R0 = 0, OFF_R1 = TILE, OFF_S0 = 2 * TILE, OFF_S1 = OFF_S0 + 2 * TILE, OFF_VEC = OFF_S1 + 2 * TILE, OFF_BAR = OFF_VEC + 2 * 64 * 4;
+constexpr int SMEM = OFF_BAR + 64 + 1024; // two resident tiles + two streamed tiles x 2 stages
 constexpr float LOG2E = 1.4426950408889634f;
 
 struct BwdParams {
@@ -46,63 +39,53 @@ struct BwdParams {
 
 __device__ __forceinline__ float ex2(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
-// SS GEMM: acc[128 x 64] = A . B^T, A a K-major [128 x 128] tile, B a K-major [64 x 128] tile
-__device__ __forceinline__ void mma_ss_kmajor(uint32_t tmem_d, uint32_t a_addr, uint32_t b_addr) {
-    constexpr uint32_t idesc = br::make_idesc_bf16(128, BS);
+// acc[64 x 64] = A . B^T over d = 128, A and B K-major [64 x 128] tiles
+__device__ __forceinline__ void mma_ss(float (&acc)[32], uint32_t a_addr, uint32_t b_addr) {
 #pragma unroll
-    for (int kk = 0; kk < D / 16; ++kk)
-        br::tc_mma_bf16(tmem_d, br::make_sw128_kmajor_desc(a_addr + (kk >> 2) * BLK + (kk & 3) * 32),
-                        br::make_sw128_kmajor_desc(b_addr + (kk >> 2) * BLKS + (kk & 3) * 32), idesc, kk != 0);
+    for (int kk = 0; kk < D / 16; ++kk) {
+        const uint32_t off = (kk >> 2) * BLK + (kk & 3) * 32;
+        br::wgmma_ss<64>(acc, br::wg_desc_k(a_addr + off), br::wg_desc_k(b_addr + off), kk != 0);
+    }
 }
-// TS GEMM: acc[128 x 128] (+)= A(tmem: 128 x 64 bf16, packed in 32 columns) . B, B = a [64 (K) x 128 (N)] row-major tile (MN-major)
-__device__ __forceinline__ void mma_ts_mnmajor(uint32_t tmem_d, uint32_t tmem_a, uint32_t b_addr, bool accumulate) {
-    constexpr uint32_t idesc = br::make_idesc_bf16_major(128, 128, 0, 1);
+// acc[64 x 128] += A(registers: 64 x 64 bf16 from the fragment f) . B, B = a [64 (K) x 128 (N)] row-major tile (MN-major)
+__device__ __forceinline__ void mma_rs(float (&acc)[64], const float (&f)[32], uint32_t b_addr) {
 #pragma unroll
-    for (int kk = 0; kk < BS / 16; ++kk)
-        br::tc_mma_bf16_ts(tmem_d, tmem_a + kk * 8, br::make_sw128_mnmajor_desc(b_addr + kk * 2048, BLKS, 1024), idesc, accumulate || kk != 0);
+    for (int kk = 0; kk < 4; ++kk) {
+        const uint32_t a[4] = {br::pack_bf16(f[8 * kk + 0], f[8 * kk + 1]), br::pack_bf16(f[8 * kk + 2], f[8 * kk + 3]),
+                               br::pack_bf16(f[8 * kk + 4], f[8 * kk + 5]), br::pack_bf16(f[8 * kk + 6], f[8 * kk + 7])};
+        br::wgmma_rs<128, 1>(acc, a, br::wg_desc_mn(b_addr + kk * 2048, BLK, 1024), 1);
+    }
 }
-__device__ __forceinline__ void tma_tile(uint8_t* dst, const CUtensorMap* tm, uint64_t* bar, int col0, int row0, int blk) {
+__device__ __forceinline__ void tma_tile(uint8_t* dst, const CUtensorMap* tm, uint64_t* bar, int col0, int row0) {
     br::tma_load_2d(dst, tm, bar, col0, row0);
-    br::tma_load_2d(dst + blk, tm, bar, col0 + 64, row0);
+    br::tma_load_2d(dst + BLK, tm, bar, col0 + 64, row0);
 }
-__device__ __forceinline__ void store_row_bf16(bf16* dst, const uint32_t (&r)[32], float mul) {
+// rows r0 and r0 + 8 of a [64 x 128] fragment -> bf16 rows (zero when `zero`)
+__device__ __forceinline__ void store_frag(bf16* base, long long ld, int row0, int n_rows, const float (&acc)[64], int r0, int cq) {
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        uint4 w;
-        w.x = br::pack_bf16(__uint_as_float(r[q * 8 + 0]) * mul, __uint_as_float(r[q * 8 + 1]) * mul);
-        w.y = br::pack_bf16(__uint_as_float(r[q * 8 + 2]) * mul, __uint_as_float(r[q * 8 + 3]) * mul);
-        w.z = br::pack_bf16(__uint_as_float(r[q * 8 + 4]) * mul, __uint_as_float(r[q * 8 + 5]) * mul);
-        w.w = br::pack_bf16(__uint_as_float(r[q * 8 + 6]) * mul, __uint_as_float(r[q * 8 + 7]) * mul);
-        *reinterpret_cast<uint4*>(dst + q * 8) = w;
+    for (int hh = 0; hh < 2; ++hh) {
+        const int r = row0 + r0 + 8 * hh;
+        if (r >= n_rows) continue;
+        bf16* dst = base + (long long)r * ld;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) *reinterpret_cast<uint32_t*>(dst + 8 * i + cq) = br::pack_bf16(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
     }
 }
 
 // =====================================================================================================================
 // dq kernel
 // =====================================================================================================================
-constexpr int NSTK = 4;                   // dq kernel: a K tile is held until dQ += dS K of ITS tile retires (two tiles after its scores) -> one more stage
-constexpr int DQ_OFF_Q = 0, DQ_OFF_DO = TILE, DQ_OFF_K = 2 * TILE, DQ_OFF_V = DQ_OFF_K + NSTK * TILES, DQ_OFF_RED = DQ_OFF_V + NST * TILES,
-              DQ_OFF_BAR = DQ_OFF_RED + 256 * 4;
-constexpr int DQ_SMEM = DQ_OFF_BAR + 256 + 1024;
-
 __global__ void __launch_bounds__(NTHREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                    const __grid_constant__ CUtensorMap tmDO, const BwdParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    float* s_red = reinterpret_cast<float*>(smem + DQ_OFF_RED);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + DQ_OFF_BAR);
+    float* s_red = reinterpret_cast<float*>(smem + OFF_VEC);              // [2][64] delta halves
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
     uint64_t* qdo_full = bars;                    // 1
-    uint64_t* k_full = bars + 1;                  // NSTK
-    uint64_t* v_full = k_full + NSTK;             // NST
-    uint64_t* k_empty = v_full + NST;             // NSTK
-    uint64_t* v_empty = k_empty + NSTK;           // NST
-    uint64_t* sdp_full = v_empty + NST;           // 3: S and dP of tile t (buffer t % 3) ready
-    uint64_t* ds_full = sdp_full + 3;             // 3: dS of tile t in TMEM
-    uint64_t* dq_final = ds_full + 3;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(dq_final + 1);
+    uint64_t* kv_full = bars + 1;                 // 2
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int qb = gridDim.x - 1 - blockIdx.x;
     const int h = blockIdx.y, b = blockIdx.z;
     const int hk = h / (p.Hq / p.Hkv);
@@ -110,360 +93,210 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     const int ks = p.kv_start ? p.kv_start[b] : 0;
     const int ke = p.kv_end ? p.kv_end[b] : p.L;
     const int last_key = min(ke - 1, q0 + BT - 1);
-    const int jb_lo = ks / BS;
-    int jb_hi = last_key >= 0 ? last_key / BS : -1;
+    const int jb_lo = ks / BT;
+    int jb_hi = last_key >= 0 ? last_key / BT : -1;
     if (ke <= ks) jb_hi = jb_lo - 1;
     const int n_tiles = max(0, jb_hi - jb_lo + 1);
 
-    if (warp == 0 && lane == 0) {
+    auto load_kv = [&](int t) {
+        const int st = t & 1, row_k = b * p.L + (jb_lo + t) * BT;
+        br::mbar_expect_tx(&kv_full[st], 2 * TILE);
+        tma_tile(smem + OFF_S0 + st * TILE, &tmK, &kv_full[st], hk * D, row_k);
+        tma_tile(smem + OFF_S1 + st * TILE, &tmV, &kv_full[st], hk * D, row_k);
+    };
+    if (tid == 0) {
         br::tma_prefetch_desc(&tmQ); br::tma_prefetch_desc(&tmK); br::tma_prefetch_desc(&tmV); br::tma_prefetch_desc(&tmDO);
-        br::mbar_init(qdo_full, 1);
-        for (int s = 0; s < NSTK; ++s) { br::mbar_init(&k_full[s], 1); br::mbar_init(&k_empty[s], 1); }
-        for (int s = 0; s < NST; ++s) { br::mbar_init(&v_full[s], 1); br::mbar_init(&v_empty[s], 1); }
-        for (int s = 0; s < 3; ++s) { br::mbar_init(&sdp_full[s], 1); br::mbar_init(&ds_full[s], 4); }
-        br::mbar_init(dq_final, 1);
+        br::mbar_init(qdo_full, 1); br::mbar_init(&kv_full[0], 1); br::mbar_init(&kv_full[1], 1);
         br::mbar_fence_init();
-    }
-    if (warp == 1) { br::tmem_alloc(tmem_slot, 512); br::tmem_relinquish(); }
-    br::tc_fence_before();
-    __syncthreads();
-    br::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    // S[3], dP[3] (64 columns each), dQ (128): THREE score buffers for two element-wise groups, so the scores of the tile a group
-    // turns to next were issued a whole tile period earlier (with two buffers they could only be issued once that group had released
-    // its buffer, and every tile began with a wait for the tensor pipe)
-    const uint32_t tm_s = tmem_base, tm_dp = tmem_base + 3 * BS, tm_dq = tmem_base + 6 * BS;
-
-    if (warp == 0) {
-        if (lane == 0 && n_tiles > 0) {
+        if (n_tiles > 0) {
             const int row_q = b * p.L + q0;
             br::mbar_expect_tx(qdo_full, 2 * TILE);
-            tma_tile(smem + DQ_OFF_Q, &tmQ, qdo_full, h * D, row_q, BLK);
-            tma_tile(smem + DQ_OFF_DO, &tmDO, qdo_full, h * D, row_q, BLK);
-            int sk = 0, sv = 0; uint32_t phk = 0, phv = 0;
-            for (int t = 0; t < n_tiles; ++t) {
-                const int row_k = b * p.L + (jb_lo + t) * BS;
-                br::mbar_wait(&k_empty[sk], phk ^ 1);
-                br::mbar_expect_tx(&k_full[sk], TILES);
-                tma_tile(smem + DQ_OFF_K + sk * TILES, &tmK, &k_full[sk], hk * D, row_k, BLKS);
-                br::mbar_wait(&v_empty[sv], phv ^ 1);
-                br::mbar_expect_tx(&v_full[sv], TILES);
-                tma_tile(smem + DQ_OFF_V + sv * TILES, &tmV, &v_full[sv], hk * D, row_k, BLKS);
-                if (++sk == NSTK) { sk = 0; phk ^= 1; }
-                if (++sv == NST) { sv = 0; phv ^= 1; }
-            }
+            tma_tile(smem + OFF_R0, &tmQ, qdo_full, h * D, row_q);
+            tma_tile(smem + OFF_R1, &tmDO, qdo_full, h * D, row_q);
+            load_kv(0);
+            if (n_tiles > 1) load_kv(1);
         }
-    } else if (warp == 1) {
-        if (lane == 0 && n_tiles > 0) {
-            const uint32_t q_addr = br::smem_u32(smem + DQ_OFF_Q), do_addr = br::smem_u32(smem + DQ_OFF_DO);
-            br::mbar_wait(qdo_full, 0);
-            br::tc_fence_after();
-            int sk = 0, sv = 0; uint32_t phk = 0, phv = 0;   // ring positions of tile t
-            int su = 0;                                      // K ring position of tile t - 2
-            for (int t = 0; t < n_tiles + 2; ++t) {
-                if (t < n_tiles) {
-                    const uint32_t k_addr = br::smem_u32(smem + DQ_OFF_K + sk * TILES), v_addr = br::smem_u32(smem + DQ_OFF_V + sv * TILES);
-                    const int b3 = t % 3;
-                    br::mbar_wait(&k_full[sk], phk);
-                    br::tc_fence_after();
-                    mma_ss_kmajor(tm_s + b3 * BS, q_addr, k_addr);                          // S = Q K^T
-                    br::mbar_wait(&v_full[sv], phv);
-                    br::tc_fence_after();
-                    mma_ss_kmajor(tm_dp + b3 * BS, do_addr, v_addr);                        // dP = dO V^T
-                    br::tc_commit(&sdp_full[b3]);
-                    br::tc_commit(&v_empty[sv]);
-                    if (++sk == NSTK) { sk = 0; phk ^= 1; }
-                    if (++sv == NST) { sv = 0; phv ^= 1; }
-                }
-                if (t >= 2) {
-                    const int u = t - 2, b3 = u % 3;
-                    br::mbar_wait(&ds_full[b3], (u / 3) & 1);
-                    br::tc_fence_after();
-                    mma_ts_mnmajor(tm_dq, tm_dp + b3 * BS, br::smem_u32(smem + DQ_OFF_K + su * TILES), u != 0);          // dQ += dS K
-                    br::tc_commit(&k_empty[su]);
-                    if (++su == NSTK) su = 0;
-                }
-            }
-            br::tc_commit(dq_final);
-        }
-    } else {
-        // element-wise group g = tiles t = g, g + 2, ...; one thread per query row (TMEM lane)
-        const int lane_grp = warp & 3;
-        const int g = (warp - 2) >> 2, col0 = g * 64;                     // col0: this group's half of the head dim for delta / the dQ store
-        const int row = lane_grp * 32 + lane;
+    }
+    // ---- delta = rowsum(dO o O) (fp32; two threads per query row, each half of the head dim, summed in a fixed order)
+    {
+        const int row = tid >> 1, half = tid & 1;
         const int i_glob = q0 + row;
-        const bool row_ok = i_glob < p.L;
-        const uint32_t lane_off = (uint32_t)(lane_grp * 32) << 16;
-        const long long tok = (long long)b * p.L + i_glob;
-        // ---- delta = rowsum(dO o O) for this query row (fp32; each group half of the head dim), published for the dk/dv kernel
         float delta = 0.f;
-        if (row_ok) {
-            const uint4* op = reinterpret_cast<const uint4*>(p.o + tok * p.ldo + (long long)h * D + col0);
-            const uint4* dp = reinterpret_cast<const uint4*>(p.dout + tok * p.lddo + (long long)h * D + col0);
-            uint4 av[D / 16], gv[D / 16];                          // all 16 loads of the row in flight at once: this prologue runs with nothing
-#pragma unroll                                                   // else resident on the SM, every dependent round trip is exposed
-            for (int c = 0; c < D / 16; ++c) { av[c] = __ldg(op + c); gv[c] = __ldg(dp + c); }
+        if (i_glob < p.L) {
+            const long long tok = (long long)b * p.L + i_glob;
+            const uint4* op = reinterpret_cast<const uint4*>(p.o + tok * p.ldo + (long long)h * D + half * 64);
+            const uint4* dp = reinterpret_cast<const uint4*>(p.dout + tok * p.lddo + (long long)h * D + half * 64);
+            uint4 av[8], gv[8];
 #pragma unroll
-            for (int c = 0; c < D / 16; ++c) {
+            for (int c = 0; c < 8; ++c) { av[c] = __ldg(op + c); gv[c] = __ldg(dp + c); }
+#pragma unroll
+            for (int c = 0; c < 8; ++c) {
                 const uint4 a = av[c], gd = gv[c];
                 const float2 a0 = br::unpack_bf16(a.x), a1 = br::unpack_bf16(a.y), a2 = br::unpack_bf16(a.z), a3 = br::unpack_bf16(a.w);
                 const float2 g0 = br::unpack_bf16(gd.x), g1 = br::unpack_bf16(gd.y), g2 = br::unpack_bf16(gd.z), g3 = br::unpack_bf16(gd.w);
                 delta += a0.x * g0.x + a0.y * g0.y + a1.x * g1.x + a1.y * g1.y + a2.x * g2.x + a2.y * g2.y + a3.x * g3.x + a3.y * g3.y;
             }
         }
-        s_red[g * 128 + row] = delta;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        delta = s_red[row] + s_red[128 + row];                          // fixed order: both threads of the row get the same value
-        if (row_ok && g == 0) p.delta[((long long)b * p.Hq + h) * p.L + i_glob] = delta;
-        const float lse2 = row_ok ? p.lse[((long long)b * p.Hq + h) * p.L + i_glob] * LOG2E : INFINITY;
-        const float delta_s = delta * p.scale;
-        for (int t = g; t < n_tiles; t += 2) {
-            const int k0 = (jb_lo + t) * BS;
-            const bool need_mask = (k0 < ks) || (k0 + BS > ke) || (k0 + BS - 1 > q0);
-            const int b3 = t % 3;
-            const uint32_t ts = tm_s + b3 * BS + lane_off, tp = tm_dp + b3 * BS + lane_off;
-            br::mbar_wait(&sdp_full[b3], (t / 3) & 1);
-            br::tc_fence_after();
-#pragma unroll
-            for (int c = 0; c < BS; c += 32) {
-                uint32_t rs[32], rp[32];
-                br::tmem_ld_32x32(ts + c, rs);
-                br::tmem_ld_32x32(tp + c, rp);
-                br::tmem_ld_wait();
-                uint32_t pk[16];
-                if (need_mask) {                                         // one branch per chunk: the arithmetic below stays one basic block
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) {
-                        const int j = k0 + c + e;
-                        if (!((j >= ks) && (j < ke) && (j <= i_glob))) rs[e] = 0xff800000u;      // -inf score -> probability 0
-                    }
-                }
-#pragma unroll
-                for (int e = 0; e < 32; e += 2) {
-                    const float x0 = fmaf(__uint_as_float(rs[e]), p.scale_log2, -lse2), x1 = fmaf(__uint_as_float(rs[e + 1]), p.scale_log2, -lse2);
-                    const float p0 = ex2(x0), p1 = ex2(x1);
-                    const float d0 = p0 * fmaf(__uint_as_float(rp[e]), p.scale, -delta_s), d1 = p1 * fmaf(__uint_as_float(rp[e + 1]), p.scale, -delta_s);
-                    pk[e >> 1] = br::pack_bf16(d0, d1);
-                }
-                br::tmem_st_32x16(tp + (c >> 1), pk);                    // dS (packed) over the first 32 of the 64 consumed dP columns
-            }
-            br::tmem_st_wait();
-            br::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) br::mbar_arrive(&ds_full[b3]);
-        }
-        bf16* dq_row = p.dq + tok * p.lddq + (long long)h * D + col0;
-        if (n_tiles > 0) {
-            br::mbar_wait(dq_final, 0);
-            br::tc_fence_after();
-#pragma unroll
-            for (int c = 0; c < 64; c += 32) {
-                uint32_t r[32];
-                br::tmem_ld_32x32(tm_dq + lane_off + col0 + c, r);
-                br::tmem_ld_wait();
-                if (row_ok) store_row_bf16(dq_row + c, r, 1.f);
-            }
-        } else if (row_ok) {
-#pragma unroll
-            for (int c = 0; c < 64; c += 8) *reinterpret_cast<uint4*>(dq_row + c) = make_uint4(0, 0, 0, 0);
-        }
+        s_red[half * 64 + row] = delta;
     }
-    br::tc_fence_before();
     __syncthreads();
-    if (warp == 1) { br::tc_fence_after(); br::tmem_dealloc(tmem_base, 512); }
+    if (tid < 64 && q0 + tid < p.L) p.delta[((long long)b * p.Hq + h) * p.L + q0 + tid] = s_red[tid] + s_red[64 + tid];
+    const int r0 = warp * 16 + (lane >> 2), cq = 2 * (lane & 3);
+    float lse2[2], delta_s[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        const int i_glob = q0 + r0 + 8 * hh;
+        lse2[hh] = i_glob < p.L ? p.lse[((long long)b * p.Hq + h) * p.L + i_glob] * LOG2E : INFINITY;
+        delta_s[hh] = (s_red[r0 + 8 * hh] + s_red[64 + r0 + 8 * hh]) * p.scale;    // same fixed order as the published value
+    }
+    float dq[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) dq[i] = 0.f;
+    const uint32_t q_addr = br::smem_u32(smem + OFF_R0), do_addr = br::smem_u32(smem + OFF_R1);
+    if (n_tiles > 0) br::mbar_wait(qdo_full, 0);
+    for (int t = 0; t < n_tiles; ++t) {
+        const int st = t & 1;
+        const int k0 = (jb_lo + t) * BT;
+        const uint32_t k_addr = br::smem_u32(smem + OFF_S0 + st * TILE), v_addr = br::smem_u32(smem + OFF_S1 + st * TILE);
+        br::mbar_wait(&kv_full[st], (t >> 1) & 1);
+        float s[32], dp[32];
+        br::wg_fence();
+        mma_ss(s, q_addr, k_addr);                                            // S = Q K^T
+        mma_ss(dp, do_addr, v_addr);                                          // dP = dO V^T
+        br::wg_commit();
+        br::wg_wait<0>();
+        br::wg_fence_operand(s);
+        br::wg_fence_operand(dp);
+        const bool need_mask = (k0 < ks) || (k0 + BT > ke) || (k0 + BT - 1 > q0);
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int x = 4 * i + 2 * hh + e;
+                    const int j = k0 + 8 * i + cq + e, ig = q0 + r0 + 8 * hh;
+                    float sv = s[x];
+                    if (need_mask && !((j >= ks) && (j < ke) && (j <= ig))) sv = -INFINITY;      // -inf score -> probability 0
+                    const float pr = ex2(fmaf(sv, p.scale_log2, -lse2[hh]));
+                    s[x] = pr * fmaf(dp[x], p.scale, -delta_s[hh]);                              // dS
+                }
+        br::wg_fence();
+        mma_rs(dq, s, k_addr);                                                // dQ += dS K
+        br::wg_commit();
+        br::wg_wait<0>();
+        br::wg_fence_operand(dq);
+        __syncthreads();
+        if (tid == 0 && t + 2 < n_tiles) load_kv(t + 2);
+    }
+    store_frag(p.dq + (long long)b * p.L * p.lddq + (long long)h * D, p.lddq, q0, p.L, dq, r0, cq);
 }
 
 // =====================================================================================================================
 // dk / dv kernel
 // =====================================================================================================================
-constexpr int KV_OFF_K = 0, KV_OFF_V = TILE, KV_OFF_Q = 2 * TILE, KV_OFF_DO = KV_OFF_Q + NST * TILES, KV_OFF_VEC = KV_OFF_DO + NST * TILES,
-              KV_OFF_BAR = KV_OFF_VEC + 2 * 2 * 128 * 4;
-constexpr int KV_SMEM = KV_OFF_BAR + 256 + 1024;
-
 __global__ void __launch_bounds__(NTHREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                     const __grid_constant__ CUtensorMap tmDO, const BwdParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    float* s_vec = reinterpret_cast<float*>(smem + KV_OFF_VEC);           // [group][parity][0..63: lse*log2e, 64..127: delta*scale]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + KV_OFF_BAR);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
     uint64_t* kv_full = bars;                     // 1
-    uint64_t* q_full = bars + 1;                  // NST
-    uint64_t* do_full = q_full + NST;
-    uint64_t* qdo_empty = do_full + NST;
-    uint64_t* sdp_full = qdo_empty + NST;         // 2
-    uint64_t* pds_full = sdp_full + 2;            // 2
-    uint64_t* acc_final = pds_full + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_final + 1);
+    uint64_t* qdo_full = bars + 1;                // 2
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int jb = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
     const int GQ = p.Hq / p.Hkv;
     const int key0 = jb * BT;
     const int ks = p.kv_start ? p.kv_start[b] : 0;
     const int ke = p.kv_end ? p.kv_end[b] : p.L;
     const bool block_live = (key0 < ke) && (key0 + BT > ks) && (key0 < p.L);
-    const int n_ib = (p.L + BS - 1) / BS;                                 // 64-query tiles
-    const int ib_lo = key0 / BS;                                          // causal: the first query tile that sees a key of this block
+    const int n_ib = (p.L + BT - 1) / BT;                                 // 64-query tiles
+    const int ib_lo = key0 / BT;                                          // causal: the first query tile that sees a key of this block
     const int per_head = n_ib - ib_lo;
     const int iters = block_live ? GQ * per_head : 0;
 
-    if (warp == 0 && lane == 0) {
+    auto load_qdo = [&](int it) {
+        const int st = it & 1;
+        const int h = hk * GQ + it / per_head, ib = ib_lo + it % per_head;
+        const int row_q = b * p.L + ib * BT;
+        br::mbar_expect_tx(&qdo_full[st], 2 * TILE);
+        tma_tile(smem + OFF_S0 + st * TILE, &tmQ, &qdo_full[st], h * D, row_q);
+        tma_tile(smem + OFF_S1 + st * TILE, &tmDO, &qdo_full[st], h * D, row_q);
+    };
+    if (tid == 0) {
         br::tma_prefetch_desc(&tmQ); br::tma_prefetch_desc(&tmK); br::tma_prefetch_desc(&tmV); br::tma_prefetch_desc(&tmDO);
-        br::mbar_init(kv_full, 1);
-        for (int s = 0; s < NST; ++s) { br::mbar_init(&q_full[s], 1); br::mbar_init(&do_full[s], 1); br::mbar_init(&qdo_empty[s], 1); }
-        for (int s = 0; s < 2; ++s) { br::mbar_init(&sdp_full[s], 1); br::mbar_init(&pds_full[s], 4); }
-        br::mbar_init(acc_final, 1);
+        br::mbar_init(kv_full, 1); br::mbar_init(&qdo_full[0], 1); br::mbar_init(&qdo_full[1], 1);
         br::mbar_fence_init();
-    }
-    if (warp == 1) { br::tmem_alloc(tmem_slot, 512); br::tmem_relinquish(); }
-    br::tc_fence_before();
-    __syncthreads();
-    br::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tm_s = tmem_base, tm_dp = tmem_base + 2 * BS, tm_dv = tmem_base + 256, tm_dk = tmem_base + 384;
-
-    if (warp == 0) {
-        if (lane == 0 && iters > 0) {
+        if (iters > 0) {
             const int row_k = b * p.L + key0;
             br::mbar_expect_tx(kv_full, 2 * TILE);
-            tma_tile(smem + KV_OFF_K, &tmK, kv_full, hk * D, row_k, BLK);
-            tma_tile(smem + KV_OFF_V, &tmV, kv_full, hk * D, row_k, BLK);
-            int s = 0; uint32_t ph = 0;
-            for (int it = 0; it < iters; ++it) {
-                const int h = hk * GQ + it / per_head, ib = ib_lo + it % per_head;
-                const int row_q = b * p.L + ib * BS;
-                br::mbar_wait(&qdo_empty[s], ph ^ 1);
-                br::mbar_expect_tx(&q_full[s], TILES);
-                tma_tile(smem + KV_OFF_Q + s * TILES, &tmQ, &q_full[s], h * D, row_q, BLKS);
-                br::mbar_expect_tx(&do_full[s], TILES);
-                tma_tile(smem + KV_OFF_DO + s * TILES, &tmDO, &do_full[s], h * D, row_q, BLKS);
-                if (++s == NST) { s = 0; ph ^= 1; }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0 && iters > 0) {
-            const uint32_t k_addr = br::smem_u32(smem + KV_OFF_K), v_addr = br::smem_u32(smem + KV_OFF_V);
-            br::mbar_wait(kv_full, 0);
-            br::tc_fence_after();
-            int s = 0; uint32_t ph = 0;
-            int su = 0;
-            for (int it = 0; it <= iters; ++it) {
-                if (it < iters) {
-                    const uint32_t q_addr = br::smem_u32(smem + KV_OFF_Q + s * TILES), do_addr = br::smem_u32(smem + KV_OFF_DO + s * TILES);
-                    br::mbar_wait(&q_full[s], ph);
-                    br::tc_fence_after();
-                    mma_ss_kmajor(tm_s + (it & 1) * BS, k_addr, q_addr);                    // S^T = K Q^T
-                    br::mbar_wait(&do_full[s], ph);
-                    br::tc_fence_after();
-                    mma_ss_kmajor(tm_dp + (it & 1) * BS, v_addr, do_addr);                  // dP^T = V dO^T
-                    br::tc_commit(&sdp_full[it & 1]);
-                    if (++s == NST) { s = 0; ph ^= 1; }
-                }
-                if (it >= 1) {
-                    const int u = it - 1;
-                    const uint32_t q_addr = br::smem_u32(smem + KV_OFF_Q + su * TILES), do_addr = br::smem_u32(smem + KV_OFF_DO + su * TILES);
-                    br::mbar_wait(&pds_full[u & 1], (u >> 1) & 1);
-                    br::tc_fence_after();
-                    mma_ts_mnmajor(tm_dv, tm_s + (u & 1) * BS, do_addr, u != 0);            // dV += P^T dO
-                    mma_ts_mnmajor(tm_dk, tm_dp + (u & 1) * BS, q_addr, u != 0);            // dK += dS^T Q
-                    br::tc_commit(&qdo_empty[su]);
-                    if (++su == NST) su = 0;
-                }
-            }
-            br::tc_commit(acc_final);
-        }
-    } else {
-        // element-wise group g = iterations it = g, g + 2, ...; one thread per key row (TMEM lane), 64 query columns
-        const int lane_grp = warp & 3;
-        const int g = (warp - 2) >> 2, col0 = g * 64;                      // col0: this group's half of the head dim in the final store
-        const int row = lane_grp * 32 + lane;                              // key row inside the tile == TMEM lane
-        const int eg = threadIdx.x - 64 - g * 128;                         // 0..127 inside the group
-        const int j_glob = key0 + row;
-        const bool key_ok = (j_glob >= ks) && (j_glob < ke);
-        const uint32_t lane_off = (uint32_t)(lane_grp * 32) << 16;
-        // per-query vectors of this group's NEXT iteration, one element per thread (0..63: lse, 64..127: delta), fetched one iteration ahead
-        auto fetch_vec = [&](int it) -> float {
-            const int h = hk * GQ + it / per_head, ib = ib_lo + it % per_head;
-            const int i = ib * BS + (eg & 63);
-            if (it < iters && i < p.L) {
-                const long long off = ((long long)b * p.Hq + h) * p.L + i;
-                return eg < 64 ? __ldg(p.lse + off) * LOG2E : __ldg(p.delta + off) * p.scale;
-            }
-            return eg < 64 ? INFINITY : 0.f;
-        };
-        float nv = fetch_vec(g);
-        for (int it = g; it < iters; it += 2) {
-            const int ib = ib_lo + it % per_head;
-            const int q0 = ib * BS;
-            float* v_l2 = s_vec + (g * 2 + ((it >> 1) & 1)) * 128; float* v_ds = v_l2 + 64;
-            v_l2[eg] = nv;                                                 // eg >= 64 lands in v_ds[eg - 64]
-            nv = fetch_vec(it + 2);
-            if (g == 0) asm volatile("bar.sync 1, 128;" ::: "memory"); else asm volatile("bar.sync 2, 128;" ::: "memory");
-            const bool need_mask = (q0 < key0 + BT - 1) || (key0 < ks) || (key0 + BT > ke) || (q0 + BS > p.L);
-            const uint32_t ts = tm_s + g * BS + lane_off, tp = tm_dp + g * BS + lane_off;
-            br::mbar_wait(&sdp_full[g], (it >> 1) & 1);
-            br::tc_fence_after();
-#pragma unroll
-            for (int c = 0; c < BS; c += 32) {
-                uint32_t rs[32], rp[32];
-                br::tmem_ld_32x32(ts + c, rs);
-                br::tmem_ld_32x32(tp + c, rp);
-                br::tmem_ld_wait();
-                uint32_t pk[16], dk_[16];
-                if (need_mask) {                                         // one branch per chunk: the arithmetic below stays one basic block
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) {
-                        const int i = q0 + c + e;
-                        if (!(key_ok && j_glob <= i)) rs[e] = 0xff800000u;                       // -inf score (i >= L rows carry lse = +inf)
-                    }
-                }
-#pragma unroll
-                for (int e = 0; e < 32; e += 4) {
-                    const float4 l4 = *reinterpret_cast<const float4*>(v_l2 + c + e), d4 = *reinterpret_cast<const float4*>(v_ds + c + e);
-                    const float ll[4] = {l4.x, l4.y, l4.z, l4.w}, dd[4] = {d4.x, d4.y, d4.z, d4.w};
-                    float pr[4], dsv[4];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        pr[u] = ex2(fmaf(__uint_as_float(rs[e + u]), p.scale_log2, -ll[u]));
-                        dsv[u] = pr[u] * fmaf(__uint_as_float(rp[e + u]), p.scale, -dd[u]);
-                    }
-                    pk[e >> 1] = br::pack_bf16(pr[0], pr[1]); pk[(e >> 1) + 1] = br::pack_bf16(pr[2], pr[3]);
-                    dk_[e >> 1] = br::pack_bf16(dsv[0], dsv[1]); dk_[(e >> 1) + 1] = br::pack_bf16(dsv[2], dsv[3]);
-                }
-                br::tmem_st_32x16(ts + (c >> 1), pk);                      // P^T (packed) over the first 32 of the 64 consumed S^T columns
-                br::tmem_st_32x16(tp + (c >> 1), dk_);                     // dS^T over the consumed dP^T columns
-            }
-            br::tmem_st_wait();
-            br::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) br::mbar_arrive(&pds_full[g]);
-        }
-        const bool row_ok = j_glob < p.L;
-        const long long tok = (long long)b * p.L + j_glob;
-        bf16* dk_row = p.dk + tok * p.lddk + (long long)hk * D + col0;
-        bf16* dv_row = p.dv + tok * p.lddv + (long long)hk * D + col0;
-        if (iters > 0) {
-            br::mbar_wait(acc_final, 0);
-            br::tc_fence_after();
-#pragma unroll
-            for (int c = 0; c < 64; c += 32) {
-                uint32_t r[32];
-                br::tmem_ld_32x32(tm_dv + lane_off + col0 + c, r);
-                br::tmem_ld_wait();
-                if (row_ok) store_row_bf16(dv_row + c, r, 1.f);
-                br::tmem_ld_32x32(tm_dk + lane_off + col0 + c, r);
-                br::tmem_ld_wait();
-                if (row_ok) store_row_bf16(dk_row + c, r, 1.f);
-            }
-        } else if (row_ok) {
-#pragma unroll
-            for (int c = 0; c < 64; c += 8) { *reinterpret_cast<uint4*>(dk_row + c) = make_uint4(0, 0, 0, 0); *reinterpret_cast<uint4*>(dv_row + c) = make_uint4(0, 0, 0, 0); }
+            tma_tile(smem + OFF_R0, &tmK, kv_full, hk * D, row_k);
+            tma_tile(smem + OFF_R1, &tmV, kv_full, hk * D, row_k);
+            load_qdo(0);
+            if (iters > 1) load_qdo(1);
         }
     }
-    br::tc_fence_before();
     __syncthreads();
-    if (warp == 1) { br::tc_fence_after(); br::tmem_dealloc(tmem_base, 512); }
+    const int r0 = warp * 16 + (lane >> 2), cq = 2 * (lane & 3);
+    bool key_ok[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) { const int j = key0 + r0 + 8 * hh; key_ok[hh] = (j >= ks) && (j < ke); }
+    float dk[64], dv[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) { dk[i] = 0.f; dv[i] = 0.f; }
+    const uint32_t k_addr = br::smem_u32(smem + OFF_R0), v_addr = br::smem_u32(smem + OFF_R1);
+    if (iters > 0) br::mbar_wait(kv_full, 0);
+    for (int it = 0; it < iters; ++it) {
+        const int st = it & 1;
+        const int h = hk * GQ + it / per_head, ib = ib_lo + it % per_head;
+        const int q0 = ib * BT;
+        // per-query vectors of this thread's 16 columns (queries beyond L carry lse = +inf: probability 0)
+        float l2[16], dd[16];
+#pragma unroll
+        for (int c = 0; c < 16; ++c) {
+            const int i = q0 + 8 * (c >> 1) + cq + (c & 1);
+            const long long off = ((long long)b * p.Hq + h) * p.L + i;
+            l2[c] = i < p.L ? __ldg(p.lse + off) * LOG2E : INFINITY;
+            dd[c] = i < p.L ? __ldcg(p.delta + off) * p.scale : 0.f;
+        }
+        const uint32_t q_addr = br::smem_u32(smem + OFF_S0 + st * TILE), do_addr = br::smem_u32(smem + OFF_S1 + st * TILE);
+        br::mbar_wait(&qdo_full[st], (it >> 1) & 1);
+        float s[32], dp[32];
+        br::wg_fence();
+        mma_ss(s, k_addr, q_addr);                                            // S^T = K Q^T
+        mma_ss(dp, v_addr, do_addr);                                          // dP^T = V dO^T
+        br::wg_commit();
+        br::wg_wait<0>();
+        br::wg_fence_operand(s);
+        br::wg_fence_operand(dp);
+        const bool need_mask = (q0 < key0 + BT - 1) || (key0 < ks) || (key0 + BT > ke);
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int x = 4 * i + 2 * hh + e, c = 2 * i + e;
+                    const int qi = q0 + 8 * i + cq + e, j = key0 + r0 + 8 * hh;
+                    float sv = s[x];
+                    if (need_mask && !(key_ok[hh] && j <= qi)) sv = -INFINITY;
+                    const float pr = ex2(fmaf(sv, p.scale_log2, -l2[c]));
+                    s[x] = pr;                                                                   // P^T
+                    dp[x] = pr * fmaf(dp[x], p.scale, -dd[c]);                                   // dS^T
+                }
+        br::wg_fence();
+        mma_rs(dv, s, do_addr);                                               // dV += P^T dO
+        mma_rs(dk, dp, q_addr);                                               // dK += dS^T Q
+        br::wg_commit();
+        br::wg_wait<0>();
+        br::wg_fence_operand(dv);
+        br::wg_fence_operand(dk);
+        __syncthreads();
+        if (tid == 0 && it + 2 < iters) load_qdo(it + 2);
+    }
+    store_frag(p.dk + (long long)b * p.L * p.lddk + (long long)hk * D, p.lddk, key0, p.L, dk, r0, cq);
+    store_frag(p.dv + (long long)b * p.L * p.lddv + (long long)hk * D, p.lddv, key0, p.L, dv, r0, cq);
 }
 
 }  // namespace
@@ -481,27 +314,23 @@ int br_attn_bwd_tc5_impl(const void* q, int64_t ldq, const void* k, int64_t ldk,
                  "attn_bwd: strides must be multiples of 8 elements");
     BR_CHECK_ARG(((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)o | (uintptr_t)dout | (uintptr_t)dq | (uintptr_t)dk | (uintptr_t)dv) % 16 == 0,
                  "attn_bwd: tensors must be 16-byte aligned");
-    CUtensorMap tq, tk, tv, tdo, tq_s, tk_s, tv_s, tdo_s;          // 128-row boxes (resident tiles) and 64-row boxes (streamed tiles)
+    CUtensorMap tq, tk, tv, tdo;                                     // 64-row boxes
     int rc;
     const uint64_t rows = (uint64_t)B * L;
     if ((rc = br_make_tmap_2d_bf16(&tq, q, rows, (uint64_t)n_q_heads * D, ldq, BT))) return rc;
     if ((rc = br_make_tmap_2d_bf16(&tk, k, rows, (uint64_t)n_kv_heads * D, ldk, BT))) return rc;
     if ((rc = br_make_tmap_2d_bf16(&tv, v, rows, (uint64_t)n_kv_heads * D, ldv, BT))) return rc;
     if ((rc = br_make_tmap_2d_bf16(&tdo, dout, rows, (uint64_t)n_q_heads * D, lddo, BT))) return rc;
-    if ((rc = br_make_tmap_2d_bf16(&tq_s, q, rows, (uint64_t)n_q_heads * D, ldq, BS))) return rc;
-    if ((rc = br_make_tmap_2d_bf16(&tk_s, k, rows, (uint64_t)n_kv_heads * D, ldk, BS))) return rc;
-    if ((rc = br_make_tmap_2d_bf16(&tv_s, v, rows, (uint64_t)n_kv_heads * D, ldv, BS))) return rc;
-    if ((rc = br_make_tmap_2d_bf16(&tdo_s, dout, rows, (uint64_t)n_q_heads * D, lddo, BS))) return rc;
     static bool done = false;
     if (!done) {
-        BR_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DQ_SMEM));
-        BR_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, KV_SMEM));
+        BR_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+        BR_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
         done = true;
     }
     const int nb = (L + BT - 1) / BT;
-    attn_bwd_dq_kernel<<<dim3(nb, n_q_heads, B), NTHREADS, DQ_SMEM, st>>>(tq, tk_s, tv_s, tdo, p);
+    attn_bwd_dq_kernel<<<dim3(nb, n_q_heads, B), NTHREADS, SMEM, st>>>(tq, tk, tv, tdo, p);
     BR_CHECK_LAUNCH();
-    attn_bwd_dkv_kernel<<<dim3(nb, n_kv_heads, B), NTHREADS, KV_SMEM, st>>>(tq_s, tk, tv, tdo_s, p);
+    attn_bwd_dkv_kernel<<<dim3(nb, n_kv_heads, B), NTHREADS, SMEM, st>>>(tq, tk, tv, tdo, p);
     BR_CHECK_LAUNCH();
     return BR_OK;
 }

@@ -1,5 +1,5 @@
-// C entry point of the flash-attention forward (br_attn_fwd): argument checks + dispatch to the tcgen05 / TMEM kernel in
-// attn_fwd_tc5.cu.  (Round 1's mma.sync kernel lived here; it was removed once the tcgen05 kernel passed the same parity tests.)
+// C entry point of the flash-attention forward (br_attn_fwd): argument checks + dispatch to the wgmma / TMA kernel in
+// attn_fwd_tc5.cu.
 #include "br_common.cuh"
 #include "../../include/bioreason_b200.h"
 

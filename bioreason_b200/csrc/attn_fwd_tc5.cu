@@ -1,31 +1,24 @@
-// Flash attention forward on tcgen05 / TMEM / TMA (sm_100a): causal GQA decoder rows (D=128) and bidirectional encoder rows (D=64).
+// Flash attention forward on wgmma / TMA (sm_90a): causal GQA decoder rows (D=128) and bidirectional encoder rows (D=64).
 // Replaces the SDPA call HF reaches from Qwen3Attention.forward (qwen3/modeling_qwen3.py:255-263) and EsmSelfAttention.forward
-// (esm/modeling_esm.py:349-359); SURVEY.md §2.3 K1/K5.  Same contract as the previous mma.sync kernel: dense [B, L] token-major rows,
-// row b attends keys j in [kv_start[b], kv_end[b]) (one contiguous window: left pads / post-EOS tail are outside), j <= i when causal;
-// optional log-sum-exp output for the backward.
+// (esm/modeling_esm.py:349-359); SURVEY.md §2.3 K1/K5.  Dense [B, L] token-major rows, row b attends keys j in
+// [kv_start[b], kv_end[b]) (one contiguous window: left pads / post-EOS tail are outside), j <= i when causal; optional
+// log-sum-exp output for the backward.
 //
-// One CTA = one 128-query tile of one (batch row, query head); 192 threads, TWO CTAs per SM (256 TMEM columns, ~97 KB of shared memory each):
-//   warp 0      TMA producer : Q tile once; K and V tiles (64 keys x D, 128B-swizzled 64-column boxes) through 2- or 3-stage rings
-//   warp 1      MMA issuer   : S_j = Q K_j^T   (tcgen05.mma M=128 N=64, both operands K-major in shared memory) into one of two
-//                              TMEM score buffers, then O += P_{j-1} V_{j-1} with P read from TENSOR MEMORY (A operand in TMEM, packed
-//                              bf16 written by the softmax threads over the score buffer they just consumed) and V as an MN-major
-//                              shared-memory operand (the TMA tile [keys, d] as it lands: no transposed copy of V anywhere).
-//                              QK_j is issued before PV_{j-1}, so the tensor pipe computes the next scores while tile j-1 is in softmax.
-//   warps 2..5  softmax      : one thread per query row (TMEM lane), 64 score columns: tcgen05.ld, mask, running max in the log2 domain with
-//                              LAZY rescaling (the accumulator row in TMEM is only rescaled when the max grew by more than 2^8, so
-//                              the O round trip through registers leaves the critical path), exp2, bf16 pack, tcgen05.st of P, row sums
-//                              in fp32; at the end O / l -> bf16 rows, LSE.
-// Why two small CTAs instead of one large one: the per-tile chain (scores ready -> tcgen05.ld -> max -> exp2 -> tcgen05.st -> P ready -> MMA)
-// is a latency chain, and the exp2 work (16 k MUFU operations per 128 x 128 scores = 1024 clocks per SM) is as long as the two MMAs of
-// the tile.  One CTA with 256 softmax threads in lock-step (row-max exchange through shared memory + a 256-thread barrier per tile) ran
-// the tensor pipe at 26 %: its warps all sat in the same phase at the same time.  Two independent CTAs with 64-key tiles need no
-// exchange (one thread owns a whole row of the tile) and interleave their phases on the SM's MUFU / tensor / TMEM-load units.
+// One CTA = one warpgroup = one 64-query tile of one (batch row, query head); 80 KB of shared memory at D = 128 (two CTAs per SM),
+// 48 KB at D = 64 (four).  Thread 0 issues the TMA
+// loads: the Q tile once, K and V tiles (64 keys x D, 128B-swizzled 64-column boxes) through a two-stage ring, so tile t+1 lands
+// while tile t is computed.  Per key tile:
+//   S = Q K^T      wgmma m64n64k16, both operands K-major in shared memory, scores in registers
+//   softmax        online, in registers: a quad of lanes shares a query row (shuffle reductions), exp2 in the log2 domain
+//   O += P V       wgmma m64nDk16 with P as the REGISTER A operand (the score fragment re-packed to bf16, no shared-memory
+//                  round trip) and V as an MN-major shared-memory operand (the TMA tile [keys, d] as it lands: no transposed copy)
 #include "br_common.cuh"
 #include "../../include/bioreason_b200.h"
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int BM = 128, BN = 64, NTHREADS = 192;           // warp 0 TMA, warp 1 MMA, warps 2..5 softmax (one thread per query row)
+constexpr int BM = 64, BN = 64, NTHREADS = 128;
 
 struct FwdParams {
     bf16* o; long long ldo;
@@ -40,17 +33,13 @@ __device__ __forceinline__ float ex2(float x) { float y; asm("ex2.approx.ftz.f32
 template <int D>
 struct SL {
     static constexpr int NB = D / 64;                  // 64-column (128-byte) swizzled blocks per row
-    static constexpr int BLKQ = BM * 128;              // bytes of one [128 rows x 64 cols] block of Q
-    static constexpr int BLKK = BN * 128;              // bytes of one [64 keys x 64 cols] block of K / V
-    static constexpr int TILEQ = NB * BLKQ;
-    static constexpr int TILEK = NB * BLKK;
-    static constexpr int NST = (D == 128) ? 2 : 3;     // K and V ring depth
+    static constexpr int BLK = 64 * 128;               // bytes of one [64 rows x 64 cols] block
+    static constexpr int TILE = NB * BLK;              // a [64 x D] bf16 tile
     static constexpr int OFF_Q = 0;
-    static constexpr int OFF_K = TILEQ;
-    static constexpr int OFF_V = OFF_K + NST * TILEK;
-    static constexpr int OFF_BAR = OFF_V + NST * TILEK;
-    static constexpr int TOTAL = OFF_BAR + 256 + 1024;
-    static constexpr int TMEM_COLS = 256;              // 2 x 64 score columns + D accumulator columns (192 or 256 -> 256)
+    static constexpr int OFF_K = TILE;                 // 2 stages
+    static constexpr int OFF_V = OFF_K + 2 * TILE;     // 2 stages
+    static constexpr int OFF_BAR = OFF_V + 2 * TILE;
+    static constexpr int TOTAL = OFF_BAR + 64 + 1024;
 };
 
 template <int D, bool CAUSAL>
@@ -60,18 +49,10 @@ attn_fwd_tc5_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     using L = SL<D>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::OFF_BAR);
-    uint64_t* q_full = bars;                       // 1
-    uint64_t* k_full = bars + 1;                   // NST
-    uint64_t* k_empty = k_full + L::NST;
-    uint64_t* v_full = k_empty + L::NST;
-    uint64_t* v_empty = v_full + L::NST;
-    uint64_t* s_full = v_empty + L::NST;           // 2: scores of tile j ready (MMA -> softmax)
-    uint64_t* p_full = s_full + 2;                 // 2: probabilities of tile j in TMEM, accumulator rescaled (softmax -> MMA)
-    uint64_t* pv_done = p_full + 2;                // 2: O += P_j V_j retired (MMA -> softmax, for the rescale and the final read)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_done + 2);
+    uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + L::OFF_BAR);
+    uint64_t* kv_full = q_full + 1;                // 2
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int qb = gridDim.x - 1 - blockIdx.x;     // heavy (late) causal tiles first
     const int h = blockIdx.y, b = blockIdx.z;
     const int hk = h / (p.Hq / p.Hkv);
@@ -85,189 +66,125 @@ attn_fwd_tc5_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     if (ke <= ks) jb_hi = jb_lo - 1;
     const int n_tiles = max(0, jb_hi - jb_lo + 1);
 
-    if (warp == 0 && lane == 0) {
+    auto load_kv = [&](int t) {
+        const int st = t & 1, row_k = b * p.L + (jb_lo + t) * BN;
+        br::mbar_expect_tx(&kv_full[st], 2 * L::TILE);
+#pragma unroll
+        for (int nb = 0; nb < L::NB; ++nb) {
+            br::tma_load_2d(smem + L::OFF_K + st * L::TILE + nb * L::BLK, &tmK, &kv_full[st], hk * D + nb * 64, row_k);
+            br::tma_load_2d(smem + L::OFF_V + st * L::TILE + nb * L::BLK, &tmV, &kv_full[st], hk * D + nb * 64, row_k);
+        }
+    };
+    if (tid == 0) {
         br::tma_prefetch_desc(&tmQ); br::tma_prefetch_desc(&tmK); br::tma_prefetch_desc(&tmV);
-        br::mbar_init(q_full, 1);
-        for (int s = 0; s < L::NST; ++s) { br::mbar_init(&k_full[s], 1); br::mbar_init(&k_empty[s], 1); br::mbar_init(&v_full[s], 1); br::mbar_init(&v_empty[s], 1); }
-        for (int s = 0; s < 2; ++s) { br::mbar_init(&s_full[s], 1); br::mbar_init(&p_full[s], 4); br::mbar_init(&pv_done[s], 1); }
+        br::mbar_init(q_full, 1); br::mbar_init(&kv_full[0], 1); br::mbar_init(&kv_full[1], 1);
         br::mbar_fence_init();
-    }
-    if (warp == 1) { br::tmem_alloc(tmem_slot, L::TMEM_COLS); br::tmem_relinquish(); }
-    br::tc_fence_before();
-    __syncthreads();
-    br::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_o = tmem_base + 2 * BN;
-
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        if (lane == 0 && n_tiles > 0) {
-            const int row_q = b * p.L + q0;
-            br::mbar_expect_tx(q_full, L::TILEQ);
-#pragma unroll
-            for (int nb = 0; nb < L::NB; ++nb) br::tma_load_2d(smem + L::OFF_Q + nb * L::BLKQ, &tmQ, q_full, h * D + nb * 64, row_q);
-            int s = 0; uint32_t ph = 0;
-            for (int t = 0; t < n_tiles; ++t) {
-                const int row_k = b * p.L + (jb_lo + t) * BN;
-                br::mbar_wait(&k_empty[s], ph ^ 1);
-                br::mbar_expect_tx(&k_full[s], L::TILEK);
-#pragma unroll
-                for (int nb = 0; nb < L::NB; ++nb) br::tma_load_2d(smem + L::OFF_K + s * L::TILEK + nb * L::BLKK, &tmK, &k_full[s], hk * D + nb * 64, row_k);
-                br::mbar_wait(&v_empty[s], ph ^ 1);
-                br::mbar_expect_tx(&v_full[s], L::TILEK);
-#pragma unroll
-                for (int nb = 0; nb < L::NB; ++nb) br::tma_load_2d(smem + L::OFF_V + s * L::TILEK + nb * L::BLKK, &tmV, &v_full[s], hk * D + nb * 64, row_k);
-                if (++s == L::NST) { s = 0; ph ^= 1; }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (lane == 0 && n_tiles > 0) {
-            constexpr uint32_t idesc_qk = br::make_idesc_bf16(BM, BN);
-            constexpr uint32_t idesc_pv = br::make_idesc_bf16_major(BM, D, 0, 1);          // B = V, MN-major
-            const uint32_t q_addr = br::smem_u32(smem + L::OFF_Q);
-            br::mbar_wait(q_full, 0);
-            br::tc_fence_after();
-            int s = 0; uint32_t ph = 0;          // ring position of tile t
-            int sp = 0; uint32_t php = 0;        // ring position of tile t-1
-            for (int t = 0; t <= n_tiles; ++t) {
-                if (t < n_tiles) {
-                    br::mbar_wait(&k_full[s], ph);
-                    br::tc_fence_after();
-                    const uint32_t k_addr = br::smem_u32(smem + L::OFF_K + s * L::TILEK);
-                    const uint32_t tmem_s = tmem_base + (t & 1) * BN;
-#pragma unroll
-                    for (int kk = 0; kk < D / 16; ++kk) {
-                        const uint32_t qoff = (kk >> 2) * L::BLKQ + (kk & 3) * 32, koff = (kk >> 2) * L::BLKK + (kk & 3) * 32;
-                        br::tc_mma_bf16(tmem_s, br::make_sw128_kmajor_desc(q_addr + qoff), br::make_sw128_kmajor_desc(k_addr + koff), idesc_qk, kk != 0);
-                    }
-                    br::tc_commit(&s_full[t & 1]);
-                    br::tc_commit(&k_empty[s]);
-                    if (++s == L::NST) { s = 0; ph ^= 1; }
-                }
-                if (t >= 1) {
-                    const int u = t - 1;
-                    br::mbar_wait(&p_full[u & 1], (u >> 1) & 1);
-                    br::mbar_wait(&v_full[sp], php);
-                    br::tc_fence_after();
-                    const uint32_t v_addr = br::smem_u32(smem + L::OFF_V + sp * L::TILEK);
-                    const uint32_t tmem_p = tmem_base + (u & 1) * BN;
-#pragma unroll
-                    for (int kk = 0; kk < BN / 16; ++kk) {
-                        // 16 keys = 2 groups of 8 rows (SBO = 1024 B); the D/64 blocks of 64 d-columns are L::BLKK bytes apart (LBO)
-                        const uint64_t bdesc = br::make_sw128_mnmajor_desc(v_addr + kk * 2048, L::BLKK, 1024);
-                        // P (64 keys, packed bf16 pairs) sits in the first 32 columns of the score buffer it was computed from
-                        br::tc_mma_bf16_ts(tmem_o, tmem_p + kk * 8, bdesc, idesc_pv, (u | kk) != 0);
-                    }
-                    br::tc_commit(&v_empty[sp]);
-                    br::tc_commit(&pv_done[u & 1]);
-                    if (++sp == L::NST) { sp = 0; php ^= 1; }
-                }
-            }
-        }
-    } else {
-        // ===================== softmax / correction / epilogue (warps 2..5) =====================
-        const int lane_grp = warp & 3;                        // the TMEM lane quarter this warp may access
-        const int row = lane_grp * 32 + lane;                 // query row inside the tile == TMEM lane
-        const int i_glob = q0 + row;
-        const uint32_t lane_off = (uint32_t)(lane_grp * 32) << 16;
-        float m_used = -INFINITY, l = 0.f;                    // running maximum in units of RAW scores * scale_log2
-        for (int t = 0; t < n_tiles; ++t) {
-            const int nbase = (jb_lo + t) * BN;
-            const uint32_t tmem_s = tmem_base + (t & 1) * BN + lane_off;
-            const bool need_mask = (nbase < ks) || (nbase + BN > ke) || (CAUSAL && nbase + BN - 1 > q0);
-            br::mbar_wait(&s_full[t & 1], (t >> 1) & 1);
-            br::tc_fence_after();
-            uint32_t r0[32], r1[32];
-            br::tmem_ld_32x32(tmem_s, r0);
-            br::tmem_ld_32x32(tmem_s + 32, r1);
-            br::tmem_ld_wait();
-            float mx = -INFINITY;
-            if (need_mask) {
-#pragma unroll
-                for (int e = 0; e < 32; ++e) {
-                    const int ja = nbase + e, jc = nbase + 32 + e;
-                    if (!((ja >= ks) && (ja < ke) && (!CAUSAL || ja <= i_glob))) r0[e] = 0xff800000u;      // -inf
-                    if (!((jc >= ks) && (jc < ke) && (!CAUSAL || jc <= i_glob))) r1[e] = 0xff800000u;
-                }
-            }
-#pragma unroll
-            for (int e = 0; e < 32; ++e) mx = fmaxf(mx, fmaxf(__uint_as_float(r0[e]), __uint_as_float(r1[e])));
-            const float m_new = fmaxf(m_used, mx * p.scale_log2);          // scale > 0: the max commutes with the scaling
-            // lazy rescale: keep the stale maximum while the new one is within 2^8 of it (p <= 256: exact enough in bf16 / fp32 sums)
-            const bool grow = (m_new > m_used + 8.f) || (m_used == -INFINITY && m_new > -INFINITY);
-            float alpha = 1.f;
-            if (grow) { alpha = (m_used == -INFINITY) ? 0.f : ex2(m_used - m_new); m_used = m_new; }
-            const float ms = (m_used == -INFINITY) ? 0.f : m_used;
-            float rs0 = 0.f, rs1 = 0.f;
-            uint32_t pk[32];
-#pragma unroll
-            for (int e = 0; e < 32; e += 2) {
-                const float p0 = ex2(fmaf(__uint_as_float(r0[e]), p.scale_log2, -ms)), p1 = ex2(fmaf(__uint_as_float(r0[e + 1]), p.scale_log2, -ms));
-                const float p2 = ex2(fmaf(__uint_as_float(r1[e]), p.scale_log2, -ms)), p3 = ex2(fmaf(__uint_as_float(r1[e + 1]), p.scale_log2, -ms));
-                rs0 += p0 + p1; rs1 += p2 + p3;
-                pk[e >> 1] = br::pack_bf16(p0, p1); pk[16 + (e >> 1)] = br::pack_bf16(p2, p3);
-            }
-            br::tmem_st_32x32(tmem_s, pk);                    // 64 keys of P, packed, over the first 32 of the 64 score columns just read
-            l = l * alpha + (rs0 + rs1);
-            // ---- correction of the accumulator row, only when some row of the warp moved its maximum
-            if (t > 0 && __any_sync(0xffffffffu, grow)) {
-                br::mbar_wait(&pv_done[(t - 1) & 1], ((t - 1) >> 1) & 1);
-                br::tc_fence_after();
-#pragma unroll
-                for (int c = 0; c < D; c += 32) {
-                    uint32_t r[32];
-                    br::tmem_ld_32x32(tmem_o + lane_off + c, r);
-                    br::tmem_ld_wait();
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) r[e] = __float_as_uint(__uint_as_float(r[e]) * alpha);
-                    br::tmem_st_32x32(tmem_o + lane_off + c, r);
-                }
-            }
-            br::tmem_st_wait();
-            br::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) br::mbar_arrive(&p_full[t & 1]);
-        }
-        // ---- epilogue: O / l -> bf16 row, log-sum-exp
-        bf16* orow = p.o + ((long long)b * p.L + i_glob) * p.ldo + (long long)h * D;
-        const bool row_ok = i_glob < p.L;
         if (n_tiles > 0) {
-            br::mbar_wait(&pv_done[(n_tiles - 1) & 1], ((n_tiles - 1) >> 1) & 1);
-            br::tc_fence_after();
-            const float inv = l > 0.f ? 1.f / l : 0.f;
+            br::mbar_expect_tx(q_full, L::TILE);
 #pragma unroll
-            for (int c = 0; c < D; c += 32) {
-                uint32_t r[32];
-                br::tmem_ld_32x32(tmem_o + lane_off + c, r);
-                br::tmem_ld_wait();
-                if (row_ok) {
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        uint4 w;
-                        w.x = br::pack_bf16(__uint_as_float(r[q * 8 + 0]) * inv, __uint_as_float(r[q * 8 + 1]) * inv);
-                        w.y = br::pack_bf16(__uint_as_float(r[q * 8 + 2]) * inv, __uint_as_float(r[q * 8 + 3]) * inv);
-                        w.z = br::pack_bf16(__uint_as_float(r[q * 8 + 4]) * inv, __uint_as_float(r[q * 8 + 5]) * inv);
-                        w.w = br::pack_bf16(__uint_as_float(r[q * 8 + 6]) * inv, __uint_as_float(r[q * 8 + 7]) * inv);
-                        *reinterpret_cast<uint4*>(orow + c + q * 8) = w;
-                    }
-                }
-            }
-        } else if (row_ok) {
-#pragma unroll
-            for (int c = 0; c < D; c += 8) *reinterpret_cast<uint4*>(orow + c) = make_uint4(0, 0, 0, 0);
-        }
-        if (p.lse && row_ok) {
-            const float LN2 = 0.6931471805599453f;
-            p.lse[((long long)b * p.Hq + h) * p.L + i_glob] = l > 0.f ? m_used * LN2 + logf(l) : INFINITY;
+            for (int nb = 0; nb < L::NB; ++nb) br::tma_load_2d(smem + L::OFF_Q + nb * L::BLK, &tmQ, q_full, h * D + nb * 64, b * p.L + q0);
+            load_kv(0);
+            if (n_tiles > 1) load_kv(1);
         }
     }
-
-    br::tc_fence_before();
     __syncthreads();
-    if (warp == 1) {
-        br::tc_fence_after();
-        br::tmem_dealloc(tmem_base, L::TMEM_COLS);
+
+    // fragment rows of this thread: r0 and r0 + 8 of the tile; columns 8i + cq + {0, 1}
+    const int r0 = warp * 16 + (lane >> 2), cq = 2 * (lane & 3);
+    float o_acc[D / 2];
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) o_acc[i] = 0.f;
+    float m_used[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};      // running maximum in units of RAW scores * scale_log2
+    const uint32_t q_addr = br::smem_u32(smem + L::OFF_Q);
+    if (n_tiles > 0) br::mbar_wait(q_full, 0);
+    for (int t = 0; t < n_tiles; ++t) {
+        const int st = t & 1;
+        const int nbase = (jb_lo + t) * BN;
+        const uint32_t k_addr = br::smem_u32(smem + L::OFF_K + st * L::TILE), v_addr = br::smem_u32(smem + L::OFF_V + st * L::TILE);
+        br::mbar_wait(&kv_full[st], (t >> 1) & 1);
+        float s[BN / 2];
+        br::wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < D / 16; ++kk) {
+            const uint32_t off = (kk >> 2) * L::BLK + (kk & 3) * 32;
+            br::wgmma_ss<BN>(s, br::wg_desc_k(q_addr + off), br::wg_desc_k(k_addr + off), kk != 0);
+        }
+        br::wg_commit();
+        br::wg_wait<0>();
+        br::wg_fence_operand(s);
+        const bool need_mask = (nbase < ks) || (nbase + BN > ke) || (CAUSAL && nbase + BN - 1 > q0);
+        if (need_mask) {
+#pragma unroll
+            for (int i = 0; i < BN / 8; ++i)
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int j = nbase + 8 * i + cq + e, ig = q0 + r0 + 8 * hh;
+                        if (!((j >= ks) && (j < ke) && (!CAUSAL || j <= ig))) s[4 * i + 2 * hh + e] = -INFINITY;
+                    }
+        }
+        float alpha[2], ms[2];
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            float mx = -INFINITY;
+#pragma unroll
+            for (int i = 0; i < BN / 8; ++i) mx = fmaxf(mx, fmaxf(s[4 * i + 2 * hh], s[4 * i + 2 * hh + 1]));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            const float m_new = fmaxf(m_used[hh], mx * p.scale_log2);     // scale > 0: the max commutes with the scaling
+            alpha[hh] = 1.f;
+            if (m_new > m_used[hh]) { alpha[hh] = (m_used[hh] == -INFINITY) ? 0.f : ex2(m_used[hh] - m_new); m_used[hh] = m_new; }
+            ms[hh] = (m_used[hh] == -INFINITY) ? 0.f : m_used[hh];
+        }
+        float rs[2] = {0.f, 0.f};
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const float pr = ex2(fmaf(s[4 * i + 2 * hh + e], p.scale_log2, -ms[hh]));
+                    s[4 * i + 2 * hh + e] = pr;
+                    rs[hh] += pr;
+                }
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) l[hh] = l[hh] * alpha[hh] + rs[hh];
+#pragma unroll
+        for (int i = 0; i < D / 8; ++i)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) { o_acc[4 * i + 2 * hh] *= alpha[hh]; o_acc[4 * i + 2 * hh + 1] *= alpha[hh]; }
+        br::wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < BN / 16; ++kk) {
+            const uint32_t a[4] = {br::pack_bf16(s[8 * kk + 0], s[8 * kk + 1]), br::pack_bf16(s[8 * kk + 2], s[8 * kk + 3]),
+                                   br::pack_bf16(s[8 * kk + 4], s[8 * kk + 5]), br::pack_bf16(s[8 * kk + 6], s[8 * kk + 7])};
+            // 16 keys = 2 groups of 8 rows (SBO = 1024 B); the D/64 blocks of 64 d-columns are L::BLK bytes apart (LBO)
+            br::wgmma_rs<D, 1>(o_acc, a, br::wg_desc_mn(v_addr + kk * 2048, L::BLK, 1024), 1);
+        }
+        br::wg_commit();
+        br::wg_wait<0>();
+        br::wg_fence_operand(o_acc);
+        __syncthreads();                                        // every thread's products of stage st have retired
+        if (tid == 0 && t + 2 < n_tiles) load_kv(t + 2);
+    }
+    // ---- epilogue: O / l -> bf16 rows, log-sum-exp
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        float lt = l[hh];
+        lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+        lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+        const int i_glob = q0 + r0 + 8 * hh;
+        if (i_glob >= p.L) continue;
+        const float inv = lt > 0.f ? 1.f / lt : 0.f;
+        bf16* orow = p.o + ((long long)b * p.L + i_glob) * p.ldo + (long long)h * D;
+#pragma unroll
+        for (int i = 0; i < D / 8; ++i)
+            *reinterpret_cast<uint32_t*>(orow + 8 * i + cq) = br::pack_bf16(o_acc[4 * i + 2 * hh] * inv, o_acc[4 * i + 2 * hh + 1] * inv);
+        if (p.lse && (lane & 3) == 0) {
+            const float LN2 = 0.6931471805599453f;
+            p.lse[((long long)b * p.Hq + h) * p.L + i_glob] = lt > 0.f ? m_used[hh] * LN2 + logf(lt) : INFINITY;
+        }
     }
 }
 
@@ -278,7 +195,7 @@ int launch(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, 
     static bool done = false;
     if (!done) {
         BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
-        BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100));       // two CTAs per SM
+        BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100));       // several CTAs per SM
         done = true;
     }
     dim3 grid((p.L + BM - 1) / BM, p.Hq, p.B);

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libbioreason_b200 (sm_100a only).
+// Shared device/host helpers for libbioreason_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -41,7 +41,7 @@ static inline int br_num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
     }
     return n;
 }
@@ -127,119 +127,11 @@ __device__ __forceinline__ void l2_prefetch_issue(const void* tmap, const L2Pref
     }
 }
 
-// ---------------- tcgen05 / TMEM ----------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_in_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)), "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; bf16 inputs, fp32 accumulate
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// K-major operand tile in shared memory, 128-byte swizzle, rows of 64 bf16 (=128 B), 8-row groups 1024 B apart.
-// (cute::UMMA::SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), layout SWIZZLE_128B=2 [61,64))
-__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)1 << 16;                   // LBO (unused for swizzled K-major); cute sets 1
-    d |= (uint64_t)(1024 >> 4) << 32;         // SBO = 1024 B between 8-row core-matrix groups
-    d |= (uint64_t)1 << 46;                   // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                   // SWIZZLE_128B
-    return d;
-}
-// A operand read from TMEM (lane = row, two consecutive K elements packed per 32-bit column), B from a shared-memory descriptor
-// shared -> tensor memory copy of one K = 16 slice of a 128-row operand tile (128 lanes x 256 bit = 8 columns); `sdesc` is the same
-// matrix descriptor the MMA would use for that slice.  Ordered with tcgen05.mma issued by the same thread; completion via tc_commit.
-__device__ __forceinline__ void tc_cp_128x256b(uint32_t tmem_dst, uint64_t sdesc) {
-    asm volatile("tcgen05.cp.cta_group::1.128x256b [%0], %1;" ::"r"(tmem_dst), "l"(sdesc) : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// MN-major operand tile in shared memory, 128-byte swizzle (cute canonical layout ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units):
-// rows of 64 MN-contiguous bf16 (=128 B), one row per K index, 8-row groups `sbo` bytes apart, 64-wide MN blocks `lbo` bytes apart.
-// This is what a TMA box {64 cols, k rows} of a row-major [K, MN] matrix looks like (e.g. V[keys, d] as the B operand of P.V).
-__device__ __forceinline__ uint64_t make_sw128_mnmajor_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-// kind::f16 instruction descriptor: D=f32, A=B=bf16, both K-major, M x N tile
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// same with operand majors: a_mn / b_mn = 1 selects an MN-major (transposed) shared-memory operand
-__host__ __device__ constexpr uint32_t make_idesc_bf16_major(int M, int N, int a_mn, int b_mn) {
-    return make_idesc_bf16(M, N) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16);
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i <-> TMEM lane base+i)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM, 32 lanes x N consecutive 32-bit columns (thread i <-> lane base+i)
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-        "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-        "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]),
-        "r"(r[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-        "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// generic-proxy shared-memory writes -> visible to the async proxy (tcgen05.mma / TMA reading shared memory)
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma / TMA reading shared memory)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---------------- programmatic dependent launch (PDL) ----------------
-// launch_dependents: lets the NEXT kernel in the stream start its prologue (barrier init, TMEM alloc, weight prefetch)
+// launch_dependents: lets the NEXT kernel in the stream start its prologue (barrier init, weight prefetch)
 // while this one is still running; grid_dep_wait: blocks until the PREVIOUS kernel has completed and flushed memory.
 // Everything that reads or writes data shared with earlier kernels must come after grid_dep_wait().
 __device__ __forceinline__ void launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }

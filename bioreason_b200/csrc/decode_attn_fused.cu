@@ -106,26 +106,17 @@ __device__ __forceinline__ void load_head_words(const bf16* src, int lane, uint3
     whi = __ldcg(reinterpret_cast<const unsigned int*>(src + 64 + lane * 2));
 }
 
-// row r, 16-byte chunk c (0..15) of a [rows x 128] bf16 tile in the tcgen05 operand layout: two [rows x 64] blocks (`blk` bytes apart) of
-// 128-byte rows, chunk index XOR-ed with (row & 7) -- exactly what a SWIZZLE_128B TMA box leaves in shared memory
-__device__ __forceinline__ uint8_t* umma_ptr(uint8_t* base, int blk, int r, int c) {
-    return base + (c >> 3) * blk + r * 128 + (((c & 7) ^ (r & 7)) << 4);
-}
-
-// TC5 = true: the two contractions of a tile run on tcgen05 -- S = Q K^T (SS MMA, M = 128 of which the first 32 rows are query vectors,
-// N = 64 keys) into TMEM, softmax by warp 0 (thread <-> query vector <-> TMEM lane), P written back to TMEM as packed bf16, O += P V with
-// P as the TMEM A operand and the V page tile as an MN-major B operand.  TC5 = false: the round-1 mma.sync tile loop (kept for A/B runs).
-template <int D, bool TC5>
+// The two contractions of a tile run on mma.sync m16n8k16: the M dimension here is at most 32 query vectors, below the 64 rows of
+// a Hopper warpgroup MMA.
+template <int D>
 __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, const __grid_constant__ CUtensorMap tmP) {
     constexpr int BN = 64, TILE = 64 * D * 2, NT = 64, QROWS = 32, E = D / 64;
-    constexpr int QBLK = 128 * 128, KBLK = 64 * 128;          // TC5: bytes of one [128 x 64] Q block / one [64 x 64] K or V block
     extern __shared__ __align__(128) uint8_t smem_raw[];
-    uint8_t* smem = TC5 ? reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023)) : smem_raw;
-    uint8_t* sQ = smem;                          // legacy: 32 x D;  TC5: two [128 x 64] blocks (rows >= 32 are never written: their scores are ignored)
-    uint8_t* sK = smem + (TC5 ? 2 * QBLK : QROWS * D * 2);
+    uint8_t* smem = smem_raw;
+    uint8_t* sQ = smem;                          // 32 x D
+    uint8_t* sK = smem + QROWS * D * 2;
     uint8_t* sV = sK + 2 * TILE;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * TILE);          // TC5: bar_s, bar_p, bar_o, tmem slot
-    auto qptr = [&](int s, int c) -> uint8_t* { return TC5 ? umma_ptr(sQ, QBLK, s, c) : tile_ptr<D>(sQ, s, c); };
+    auto qptr = [&](int s, int c) -> uint8_t* { return tile_ptr<D>(sQ, s, c); };
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
     STAMP(0);
@@ -161,29 +152,9 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
 
     auto tile_src = [&](const bf16* cache, int pg) { return cache + (long long)table[pg] * page_stride + (long long)kvh * 64 * D; };
     auto issue_tile = [&](int st, int pg) {
-        if constexpr (TC5) {
-            const bf16* ks_ = tile_src(p.kcache, pg); const bf16* vs_ = tile_src(p.vcache, pg);
-#pragma unroll
-            for (int i = 0; i < (64 * 16) / NT; ++i) {                 // 64 keys x 16 chunks of 16 B
-                const int c = tid + i * NT, r = c >> 4, ch = c & 15;
-                cp_async16(umma_ptr(sK + st * TILE, KBLK, r, ch), ks_ + r * D + ch * 8, true);
-                cp_async16(umma_ptr(sV + st * TILE, KBLK, r, ch), vs_ + r * D + ch * 8, true);
-            }
-        } else {
             load_tile<D, NT>(sK + st * TILE, tile_src(p.kcache, pg), D, 0, 64, tid);
             load_tile<D, NT>(sV + st * TILE, tile_src(p.vcache, pg), D, 0, 64, tid);
-        }
     };
-    // TC5: tensor memory (64 score columns + 128 accumulator columns -> 256 allocated; two CTAs per SM) and the MMA <-> softmax barriers
-    uint32_t tmem_base = 0;
-    if constexpr (TC5) {
-        if (tid == 0) { br::mbar_init(&bars[0], 1); br::mbar_init(&bars[1], 1); br::mbar_init(&bars[2], 1); br::mbar_fence_init(); }
-        if (warp == 1) { br::tmem_alloc(reinterpret_cast<uint32_t*>(&bars[3]), 256); br::tmem_relinquish(); }
-        br::tc_fence_before();
-        __syncthreads();
-        br::tc_fence_after();
-        tmem_base = *reinterpret_cast<volatile uint32_t*>(&bars[3]);
-    }
     const int pg1 = pg_lo + n_splits;
     const bool have0 = pg_lo < pg_hi, have1 = pg1 < pg_hi;
     const bool early0 = have0 && pg_lo != newest_pg, early1 = have1 && pg1 != newest_pg;
@@ -307,8 +278,8 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
     if (have1 && !early1) issue_tile(1, pg1);
     cp_async_commit();
 
-    const bool warp_live = TC5 ? (warp == 0) : (shared_pass ? (warp * 16 < rows_per_unit * p.GQ) : (warp == 0));
-    if constexpr (!TC5) {
+    const bool warp_live = shared_pass ? (warp * 16 < rows_per_unit * p.GQ) : (warp == 0);
+    {
     uint32_t qf[D / 16][4];
 #pragma unroll
     for (int kk = 0; kk < D / 16; ++kk)
@@ -414,128 +385,6 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
             if (t == 0) __stcg(p.part_lse + base, l > 0.f ? m * LN2 + logf(l) : -INFINITY);
         }
     }
-    } else {
-    // ================= tcgen05 tile loop =================
-    {
-        constexpr uint32_t idesc_qk = br::make_idesc_bf16(128, BN);
-        constexpr uint32_t idesc_pv = br::make_idesc_bf16_major(128, D, 0, 1);            // B = V page tile, MN-major
-        const uint32_t tm_s = tmem_base, tm_o = tmem_base + BN;
-        const uint32_t q_addr = br::smem_u32(sQ);
-        cp_async_wait<0>();
-        br::fence_proxy_async_smem();                                   // cp.async / st.shared writes -> visible to the tensor core
-        __syncthreads();
-        STAMP(3);
-        float m_used = -INFINITY, l = 0.f;                             // warp 0: lane <-> query vector slot <-> TMEM lane
-        int it = 0;
-        for (int pg = pg_lo; pg < pg_hi; pg += n_splits, ++it) {
-            const int st = it & 1;
-            const uint32_t ph = it & 1;
-            if (warp == 1 && lane == 0) {                               // S = Q K^T
-                const uint32_t k_addr = br::smem_u32(sK + st * TILE);
-#pragma unroll
-                for (int kk = 0; kk < D / 16; ++kk)
-                    br::tc_mma_bf16(tm_s, br::make_sw128_kmajor_desc(q_addr + (kk >> 2) * QBLK + (kk & 3) * 32),
-                                    br::make_sw128_kmajor_desc(k_addr + (kk >> 2) * KBLK + (kk & 3) * 32), idesc_qk, kk != 0);
-                br::tc_commit(&bars[0]);
-            }
-            if (warp == 0) {
-                br::mbar_wait(&bars[0], ph);
-                br::tc_fence_after();
-                const int nbase = pg * BN;
-                const bool need_mask = !shared_pass && (nbase + BN > kv_len);
-                uint32_t r0[32], r1[32];
-                br::tmem_ld_32x32(tm_s, r0);
-                br::tmem_ld_32x32(tm_s + 32, r1);
-                br::tmem_ld_wait();
-                float mx = -INFINITY;
-#pragma unroll
-                for (int e = 0; e < 32; ++e) {
-                    float a = __uint_as_float(r0[e]) * p.scale_log2, b = __uint_as_float(r1[e]) * p.scale_log2;
-                    if (need_mask) { a = (nbase + e < kv_len) ? a : -INFINITY; b = (nbase + 32 + e < kv_len) ? b : -INFINITY; }
-                    r0[e] = __float_as_uint(a); r1[e] = __float_as_uint(b);
-                    mx = fmaxf(mx, fmaxf(a, b));
-                }
-                const float m_new = fmaxf(m_used, mx);
-                const bool grow = (m_new > m_used + 8.f) || (m_used == -INFINITY && m_new > -INFINITY);   // lazy rescale (see attn_fwd_tc5.cu)
-                float alpha = 1.f;
-                if (grow) { alpha = (m_used == -INFINITY) ? 0.f : exp2f(m_used - m_new); m_used = m_new; }
-                const float ms = (m_used == -INFINITY) ? 0.f : m_used;
-                float rsum = 0.f;
-                uint32_t pk[32];
-#pragma unroll
-                for (int e = 0; e < 32; e += 2) {
-                    const float p0 = exp2f(__uint_as_float(r0[e]) - ms), p1 = exp2f(__uint_as_float(r0[e + 1]) - ms);
-                    const float p2 = exp2f(__uint_as_float(r1[e]) - ms), p3 = exp2f(__uint_as_float(r1[e + 1]) - ms);
-                    rsum += (p0 + p1) + (p2 + p3);
-                    pk[e >> 1] = br::pack_bf16(p0, p1); pk[16 + (e >> 1)] = br::pack_bf16(p2, p3);
-                }
-                l = l * alpha + rsum;
-                br::tmem_st_32x32(tm_s, pk);                            // P (64 keys, packed bf16) over the 32 first score columns
-                if (it > 0 && __any_sync(0xffffffffu, grow)) {          // O of the previous tiles is complete: bars[2] was waited below
-#pragma unroll 1
-                    for (int c = 0; c < D; c += 32) {
-                        uint32_t ro[32];
-                        br::tmem_ld_32x32(tm_o + c, ro);
-                        br::tmem_ld_wait();
-#pragma unroll
-                        for (int e = 0; e < 32; ++e) ro[e] = __float_as_uint(__uint_as_float(ro[e]) * alpha);
-                        br::tmem_st_32x32(tm_o + c, ro);
-                    }
-                }
-                br::tmem_st_wait();
-                br::tc_fence_before();
-                __syncwarp();
-                if (lane == 0) br::mbar_arrive(&bars[1]);
-            }
-            if (warp == 1 && lane == 0) {                               // O += P V
-                br::mbar_wait(&bars[1], ph);
-                br::tc_fence_after();
-                const uint32_t v_addr = br::smem_u32(sV + st * TILE);
-#pragma unroll
-                for (int kk = 0; kk < BN / 16; ++kk)
-                    br::tc_mma_bf16_ts(tm_o, tm_s + kk * 8, br::make_sw128_mnmajor_desc(v_addr + kk * 2048, KBLK, 1024), idesc_pv, (it | kk) != 0);
-                br::tc_commit(&bars[2]);
-            }
-            // the accumulate retired: stage `st` is free, O is consistent for a rescale; then prefetch the tile after next into it
-            br::mbar_wait(&bars[2], ph);
-            br::tc_fence_after();
-            if (pg + 2 * n_splits < pg_hi) issue_tile(st, pg + 2 * n_splits);
-            cp_async_commit();
-            cp_async_wait<1>();                                         // tile it+1 (requested one iteration earlier / before the loop) has landed; it+2 stays in flight
-            br::fence_proxy_async_smem();
-            __syncthreads();
-        }
-        STAMP(4);
-        // ---- partials: lane s of warp 0 owns query vector s
-        if (warp == 0) {
-            const int s_idx = lane;
-            const int rr = s_idx / p.GQ, hh = kvh * p.GQ + s_idx % p.GQ;
-            const bool ok = rr < rows_per_unit && row_base + rr < p.R && s_idx < rows_per_unit * p.GQ;
-            const float inv = l > 0.f ? 1.f / l : 0.f;
-            const long long base = ok ? ((long long)(row_base + rr) * p.Hq + hh) * p.n_slots + slot_base + split : 0;
-            float* po = p.part_o + base * D;
-            const bool any_tile = pg_lo < pg_hi;
-#pragma unroll 1
-            for (int c = 0; c < D; c += 32) {
-                uint32_t ro[32];
-                if (any_tile) { br::tmem_ld_32x32(tm_o + c, ro); br::tmem_ld_wait(); }
-                if (ok) {
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) {
-                        const float4 v4 = any_tile ? make_float4(__uint_as_float(ro[q * 4]) * inv, __uint_as_float(ro[q * 4 + 1]) * inv,
-                                                                 __uint_as_float(ro[q * 4 + 2]) * inv, __uint_as_float(ro[q * 4 + 3]) * inv)
-                                                   : make_float4(0.f, 0.f, 0.f, 0.f);
-                        __stcg(reinterpret_cast<float4*>(po + c + q * 4), v4);
-                    }
-                }
-            }
-            const float LN2 = 0.6931471805599453f;
-            if (ok) __stcg(p.part_lse + base, l > 0.f ? m_used * LN2 + logf(l) : -INFINITY);
-        }
-        br::tc_fence_before();
-        __syncthreads();
-        if (warp == 1) { br::tc_fence_after(); br::tmem_dealloc(tmem_base, 256); }
-    }
     }
     STAMP(5);
     // ---- arrival counters: one per (row, kv head).  Every item publishes its partial and arrives; the SP private items of a
@@ -547,8 +396,8 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
     //      release-reduction per row -- no CTA barrier, no fence, no returning atomic on the way out.
     __syncwarp();
     if (warp_live) {
-        const int rows_in_warp = TC5 ? rows_per_unit : 16 / p.GQ; // legacy: a warp holds 16 / GQ rows; TC5: warp 0 wrote every row of the unit
-        const int rr = shared_pass ? (TC5 ? 0 : warp * rows_in_warp) + lane : 0;
+        const int rows_in_warp = 16 / p.GQ;                         // a warp holds 16 / GQ rows
+        const int rr = shared_pass ? warp * rows_in_warp + lane : 0;
         if (lane < (shared_pass ? rows_in_warp : 1) && rr < rows_per_unit && row_base + rr < p.R)
             asm volatile("red.release.gpu.global.add.s32 [%0], 1;" ::"l"(p.counters + (row_base + rr) * p.Hkv + kvh) : "memory");
     }
@@ -662,18 +511,14 @@ int br_decode_attn_fused_pf(const void* qkv_raw, int64_t ld, const void* q_norm_
     p.out = (bf16*)out; p.ldo = ldo; p.scale_log2 = scale * 1.4426950408889634f; p.theta = theta; p.eps = eps;
     p.rope = (const float2*)rope_table; p.rope_n_pos = rope_table ? rope_n_pos : 0;
     p.dbg = g_dbg;
-    constexpr int SMEM_LEGACY = 32 * D * 2 + 4 * 64 * D * 2;
-    constexpr int SMEM_TC5 = 2 * 128 * 128 + 4 * 64 * D * 2 + 64 + 1024;
-    static const bool tc5 = getenv("BR_DECODE_ATTN_TC5") && atoi(getenv("BR_DECODE_ATTN_TC5")) != 0;        // A/B switch (default flips once validated)
-    const int SMEM = tc5 ? SMEM_TC5 : SMEM_LEGACY;
+    constexpr int SMEM = 32 * D * 2 + 4 * 64 * D * 2;
     static bool done = false;
     if (!done) {
-        BR_CHECK_CUDA(cudaFuncSetAttribute(decode_fused_kernel<D, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LEGACY));
-        BR_CHECK_CUDA(cudaFuncSetAttribute(decode_fused_kernel<D, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TC5));
+        BR_CHECK_CUDA(cudaFuncSetAttribute(decode_fused_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
         done = true;
     }
     const int items = (use_shared ? (R / G) * n_kv_heads * p.SS : 0) + R * n_kv_heads * p.SP;
-    const int per_sm = tc5 ? 2 : 3;                              // TC5: 97 KB of shared memory and 256 TMEM columns per CTA
+    const int per_sm = 3;
     BR_CHECK_ARG(items <= per_sm * br_num_sms(), "decode_attn_fused: %d work items exceed the co-resident capacity (%d per SM) the in-kernel merge relies on", items, per_sm);
     CUtensorMap tp;
     memset(&tp, 0, sizeof(tp));
@@ -683,8 +528,7 @@ int br_decode_attn_fused_pf(const void* qkv_raw, int64_t ld, const void* q_norm_
         if (rc) return rc;
         p.pf_on = 1;
     }
-    if (tc5) BR_CHECK_CUDA(br_launch_pdl(decode_fused_kernel<D, true>, dim3(items), dim3(64), (size_t)SMEM, (cudaStream_t)stream, p, tp));
-    else BR_CHECK_CUDA(br_launch_pdl(decode_fused_kernel<D, false>, dim3(items), dim3(64), (size_t)SMEM, (cudaStream_t)stream, p, tp));
+    BR_CHECK_CUDA(br_launch_pdl(decode_fused_kernel<D>, dim3(items), dim3(64), (size_t)SMEM, (cudaStream_t)stream, p, tp));
     return BR_OK;
 }
 

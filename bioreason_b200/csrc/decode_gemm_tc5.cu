@@ -1,16 +1,16 @@
-// Decode-time weight-streaming GEMM on tcgen05 (swap-AB, stream-K, persistent):  out[R, N] = X[R, K] . W[N, K]^T, R <= 32.
+// Decode-time weight-streaming GEMM on wgmma (swap-AB, stream-K, persistent):  out[R, N] = X[R, K] . W[N, K]^T, R <= 32.
 //
 // Every decode step reads every weight byte once (SURVEY.md §8d: 8 GB / step for Qwen3-4B), so the kernel is HBM-bound and is
 // built around bytes in flight, not FLOPs:
-//   * swap-AB: the weight matrix is the M operand (128 output features per UMMA, M=128), the R live rows of X are the N operand
-//     (N = 16 or 32; TMA zero-fills the rows beyond R), accumulator [128 features x N] fp32 in TMEM;
-//   * one persistent CTA per SM; a TMA producer warp keeps a 6-stage ring of 128x64 weight tiles (16 KB each, 128B-swizzled)
-//     in flight (108 KB of shared memory, so this kernel and its PDL successor co-reside on an SM; the successor fills its ring
-//     BEFORE it waits for this kernel -- weights are constant during a rollout); an MMA warp issues tcgen05.mma, 4 epilogue
-//     warps drain TMEM.  (Pulling more of the chunk into L2 ahead of time was measured SLOWER: more bytes in flight only add
+//   * swap-AB: the weight matrix is the M operand (128 output features = two m64 products), the R live rows of X are the N operand
+//     (N = 16 or 32; TMA zero-fills the rows beyond R), accumulator [128 features x N] fp32 in registers;
+//   * one persistent CTA per SM; a TMA producer warp keeps a 5-stage (R <= 16) or 4-stage ring of 128x64 weight tiles (16 KB each,
+//     128B-swizzled) in flight (<= 101 KB of shared memory, so this kernel and its PDL successor co-reside on an SM; the successor fills its ring
+//     BEFORE it waits for this kernel -- weights are constant during a rollout); one consumer warpgroup issues wgmma and runs
+//     the epilogue.  (Pulling more of the chunk into L2 ahead of time was measured SLOWER: more bytes in flight only add
 //     queueing delay to the small latency-critical messages -- partial tiles, counters, activations.);
 //   * stream-K: the (feature tile, k block) units of the whole layer are cut into equal contiguous chunks, one per CTA, so
-//     small-N layers (o_proj / down_proj: 20 feature tiles) still load all 148 SMs evenly.  A tile finished by several CTAs
+//     small-N layers (o_proj / down_proj: 20 feature tiles) still load all SMs evenly.  A tile finished by several CTAs
 //     is reduced deterministically: every contributor writes its fp32 partial tile to its own scratch slot, the last arriver
 //     (arrival counter) sums the slots in ascending CTA order and applies the epilogue -- no floating-point atomics.
 // Epilogues: bf16 store, +residual, SwiGLU over (8 gate | 8 up) feature blocks, fp32 logits.
@@ -19,10 +19,11 @@
 // scratch) goes through L2 (ld.global.cg / TMA), never through L1.
 #include "br_common.cuh"
 #include "../../include/bioreason_b200.h"
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int BM = 128, BK = 64, NTHREADS = 192;
+constexpr int BM = 128, BK = 64, NTHREADS = 160;      // warps 0..3: wgmma + epilogue (one warpgroup), warp 4: TMA producer
 
 struct SkParams {
     int R, N, K;
@@ -45,33 +46,63 @@ struct SkParams {
 
 __device__ __forceinline__ float rbf(float x) { return __bfloat162float(__float2bfloat16(x)); }
 
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
 
-// PARK: tensor memory as a second-level weight buffer.  The CTA uses 2 * BNX of the 256 TMEM columns it may take (two CTAs share an SM);
-// the rest holds NPARK weight tiles in the A-operand layout (tcgen05.cp shared -> tensor memory, consumed by the TS form of the MMA), all
-// of them filled BEFORE the dependency on the previous kernel resolves -- on top of the shared-memory ring.
-template <int BNX, bool PARK>
+template <int BNX>
 struct SL {
     static constexpr int A_BYTES = BM * BK * 2;
     static constexpr int B_BYTES = BNX * BK * 2;
     static constexpr int STAGE = A_BYTES + B_BYTES;
-#ifndef BR_SK_NSTAGE
-#define BR_SK_NSTAGE 6
-#endif
-    static constexpr int NSTAGE = PARK ? 5 : BR_SK_NSTAGE;   // 6 stages = 108 KB: two CTAs (this kernel + its PDL successor) fit one SM
-    static constexpr int TMEM_COLS = PARK ? 256 : (2 * BNX < 32 ? 32 : 2 * BNX);
-    static constexpr int NPARK = PARK ? (256 - 2 * BNX) / (BK / 2) : 0;      // a 128 x 64 bf16 tile = 32 columns
+    static constexpr int NSTAGE = BNX == 16 ? 5 : 4;         // <= 101 KB per CTA: this kernel and its PDL successor fit one SM (228 KB)
     static constexpr int TILE_BYTES = NSTAGE * STAGE;
-    static constexpr int XP_BYTES = NPARK * B_BYTES;          // activation tiles of the parked weight tiles (loaded after the dependency wait)
-    static constexpr int TOTAL = TILE_BYTES + XP_BYTES + 1024 + 1024;   // + barriers / flags / per-row rstd + alignment slack
+    static constexpr int TR_BYTES = BM * (BNX + 1) * 4;       // accumulator transpose: one feature row per epilogue thread
+    static constexpr int TOTAL = TILE_BYTES + TR_BYTES + 1024 + 1024;   // + barriers / flags / per-row rstd + alignment slack
 };
+
+// The accumulator of one 128-feature tile over `n_units` consecutive ring stages (swap-AB: the weight tile is the M operand of two
+// m64nBNXk16 wgmma products, the X tile the N operand), then transposed through shared memory so that thread et holds feature et of
+// the tile for every row (the layout the epilogue and the stream-K exchange work in).  Called by the consumer warpgroup (warps 0..3).
+template <int BNX, int RM>
+__device__ __forceinline__ void mma_tile(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, int& s, uint32_t& ph, int n_units,
+                                         int* signal_counter, float* s_tr, float (&v)[RM]) {
+    using L = SL<BNX>;
+    const int et = threadIdx.x, warp = et >> 5, lane = et & 31;
+    float acc0[BNX / 2], acc1[BNX / 2];
+#pragma unroll
+    for (int i = 0; i < BNX / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+    for (int i = 0; i < n_units; ++i) {
+        br::mbar_wait(&full_bar[s], ph);
+        if (i == n_units - 1 && signal_counter && et == 0)                    // every weight tile of this CTA is on chip
+            asm volatile("red.relaxed.gpu.global.add.s32 [%0], 1;" ::"l"(signal_counter) : "memory");
+        const uint32_t sa = br::smem_u32(smem + s * L::STAGE);
+        const uint64_t bdesc = br::wg_desc_k(sa + L::A_BYTES);
+        br::wg_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+            br::wgmma_ss<BNX>(acc0, br::wg_desc_k(sa) + 2 * k, bdesc + 2 * k, 1);
+            br::wgmma_ss<BNX>(acc1, br::wg_desc_k(sa + 64 * 128) + 2 * k, bdesc + 2 * k, 1);
+        }
+        br::wg_commit();
+        br::wg_wait<0>();
+        if (et == 0) br::mbar_arrive(&empty_bar[s]);
+        if (++s == L::NSTAGE) { s = 0; ph ^= 1; }
+    }
+    br::wg_fence_operand(acc0);
+    br::wg_fence_operand(acc1);
+    asm volatile("bar.sync 1, 128;" ::: "memory");                           // the previous tile's reads of s_tr are done
+    const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < BNX / 8; ++i)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                s_tr[(fr + 8 * hh) * (BNX + 1) + 8 * i + fc + e] = acc0[4 * i + 2 * hh + e];
+                s_tr[(64 + fr + 8 * hh) * (BNX + 1) + 8 * i + fc + e] = acc1[4 * i + 2 * hh + e];
+            }
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+#pragma unroll
+    for (int r = 0; r < RM; ++r) v[r] = s_tr[et * (BNX + 1) + r];
+}
 
 // residual values of feature f for all live rows, issued as independent L2 loads (one round trip instead of R dependent ones);
 // called BEFORE the accumulator wait so the latency hides under the weight stream
@@ -159,34 +190,24 @@ __device__ __forceinline__ void compute_row_rstd(const SkParams& p, int et, floa
 }
 
 __device__ __forceinline__ long long gtime_sk() { long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-#define SKSTAMP(k) do { if (p.dbg && (threadIdx.x == 64)) p.dbg[((long long)p.dbg_slot * 160 + blockIdx.x) * 8 + (k)] = gtime_sk(); } while (0)
+#define SKSTAMP(k) do { if (p.dbg && (threadIdx.x == 0)) p.dbg[((long long)p.dbg_slot * 160 + blockIdx.x) * 8 + (k)] = gtime_sk(); } while (0)
 
-__device__ __forceinline__ void tmem_ld_32x8(uint32_t taddr, uint32_t (&r)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr) : "memory");
-}
 
-// BNX: UMMA N (rows of X the tensor core sees, zero-filled beyond R); RM: rows the epilogue code is generated for (R <= RM <= BNX).
+// BNX: wgmma N (rows of X the tensor core sees, zero-filled beyond R); RM: rows the epilogue code is generated for (R <= RM <= BNX).
 // The epilogue runs once per CTA per launch -- straight-line, instruction-fetch-bound code -- so the common R <= 8 decode batch gets its
-// own half-size instantiation.
-template <int BNX, int RM, bool PARK>
+// own half-size instantiation.  Warps 0..3: wgmma + epilogue (one feature row per thread), warp 4: TMA producer.
+template <int BNX, int RM>
 __global__ void __launch_bounds__(NTHREADS, 1)
 skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmP,
                   const SkParams p) {
-    using L = SL<BNX, PARK>;
+    using L = SL<BNX>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* xp = smem + L::TILE_BYTES;                        // PARK: [NPARK] activation tiles
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::TILE_BYTES + L::XP_BYTES);
+    float* s_tr = reinterpret_cast<float*>(smem + L::TILE_BYTES);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::TILE_BYTES + L::TR_BYTES);
     uint64_t* empty_bar = full_bar + L::NSTAGE;
-    uint64_t* tfull_bar = empty_bar + L::NSTAGE;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint64_t* pfull_bar = tempty_bar + 2;                      // PARK: weight tile of a stage landed (parking phase)
-    uint64_t* pempty_bar = pfull_bar + L::NSTAGE;              // PARK: stage copied to tensor memory
-    uint64_t* xp_bar = pempty_bar + L::NSTAGE;                 // PARK: activation tiles of the parked weight tiles landed
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(xp_bar + 1);
-    int* s_flag = reinterpret_cast<int*>(tmem_slot + 1);
-    float* s_rs = reinterpret_cast<float*>(s_flag + 1);       // [32] per-row rstd of the folded RMSNorm
+    int* s_flag = reinterpret_cast<int*>(empty_bar + L::NSTAGE);
+    float* s_rs = reinterpret_cast<float*>(s_flag + 2);       // [32] per-row rstd of the folded RMSNorm (+ [4][32] scratch)
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int u_lo = blockIdx.x * p.chunk;
@@ -194,36 +215,20 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
 
     br::launch_dependents();
     SKSTAMP(0);
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         br::tma_prefetch_desc(&tmW);
         br::tma_prefetch_desc(&tmX);
         for (int s = 0; s < L::NSTAGE; ++s) { br::mbar_init(&full_bar[s], 1); br::mbar_init(&empty_bar[s], 1); }
-        for (int s = 0; s < 2; ++s) { br::mbar_init(&tfull_bar[s], 1); br::mbar_init(&tempty_bar[s], 4); }
-        if constexpr (PARK) {
-            for (int s = 0; s < L::NSTAGE; ++s) { br::mbar_init(&pfull_bar[s], 1); br::mbar_init(&pempty_bar[s], 1); }
-            br::mbar_init(xp_bar, 1);
-        }
         br::mbar_fence_init();
     }
-    if (warp == 1) {
-        br::tmem_alloc(tmem_slot, L::TMEM_COLS);
-        br::tmem_relinquish();
-    }
-    br::tc_fence_before();
     __syncthreads();
-    br::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    // the first n_park units of the chunk are parked in tensor memory (they are consumed first: the accumulation order is unchanged),
-    // the ring holds the units after them
     const int n_units = u_hi - u_lo;
-    const int n_park = PARK ? min(L::NPARK, max(0, n_units - L::NSTAGE)) : 0;
-    const uint32_t tmem_park = tmem_base + 2 * BNX;
 
-    if (warp == 0) {
+    if (warp == 4) {
         if (lane == 0) {
             // The weights are constant during the rollout: fill the whole ring with weight tiles BEFORE waiting for the
             // previous kernel (PDL), so the HBM stream of this layer overlaps the tail of the previous kernel.
-            const int n_pre = min(L::NSTAGE, n_units - n_park);
+            const int n_pre = min(L::NSTAGE, n_units);
             const uint64_t pol = br::make_policy_evict_first();
             if (p.gate_counter && p.gate_wait >= 0) {             // start the early loads under the previous GEMM's exchange tail, not under its stream
                 const int target = (__ldcg(p.gate_epoch) - p.gate_base) * p.gate_per_step + p.gate_wait;
@@ -237,41 +242,19 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                 if (p.w_evict_first) br::tma_load_2d_hint(dst, &tmW, bar, c0, c1, pol);
                 else br::tma_load_2d(dst, &tmW, bar, c0, c1);
             };
-            if constexpr (PARK) {
-                for (int i = 0; i < n_park; ++i) {                                   // through the ring into tensor memory (MMA thread copies)
-                    const int u = u_lo + i, tile = u / p.KB, kb = u - tile * p.KB;
-                    const int st = i % L::NSTAGE, use = i / L::NSTAGE;
-                    if (use > 0) br::mbar_wait(&pempty_bar[st], (use - 1) & 1);
-                    br::mbar_expect_tx(&pfull_bar[st], L::A_BYTES);
-                    load_w(smem + st * L::STAGE, &pfull_bar[st], kb * BK, tile * BM);
-                }
-            }
             for (int i = 0; i < n_pre; ++i) {
-                const int u = u_lo + n_park + i, tile = u / p.KB, kb = u - tile * p.KB;
-                if constexpr (PARK) {                                                // the stage may still hold a tile on its way to tensor memory
-                    const int uses = (n_park - i + L::NSTAGE - 1) / L::NSTAGE;       // parked tiles that went through stage i
-                    if (i < n_park && uses > 0) br::mbar_wait(&pempty_bar[i], (uses - 1) & 1);
-                }
+                const int u = u_lo + i, tile = u / p.KB, kb = u - tile * p.KB;
                 br::mbar_expect_tx(&full_bar[i], L::STAGE);
                 load_w(smem + i * L::STAGE, &full_bar[i], kb * BK, tile * BM);
             }
             if (p.pf_on) br::l2_prefetch_issue(&tmP, p.pf, blockIdx.x, gridDim.x);     // a LATER GEMM's tiles -> L2 (HBM is otherwise idle here)
             br::grid_dep_wait();
-            if constexpr (PARK) {
-                if (n_park > 0) {
-                    br::mbar_expect_tx(xp_bar, n_park * L::B_BYTES);
-                    for (int i = 0; i < n_park; ++i) {
-                        const int u = u_lo + i, tile = u / p.KB, kb = u - tile * p.KB;
-                        br::tma_load_2d(xp + i * L::B_BYTES, &tmX, xp_bar, kb * BK, 0);
-                    }
-                }
-            }
             for (int i = 0; i < n_pre; ++i) {
-                const int u = u_lo + n_park + i, tile = u / p.KB, kb = u - tile * p.KB;
+                const int u = u_lo + i, tile = u / p.KB, kb = u - tile * p.KB;
                 br::tma_load_2d(smem + i * L::STAGE + L::A_BYTES, &tmX, &full_bar[i], kb * BK, 0);
             }
             int s = n_pre % L::NSTAGE; uint32_t ph = (n_pre == L::NSTAGE) ? 1u : 0u;
-            for (int u = u_lo + n_park + n_pre; u < u_hi; ++u) {
+            for (int u = u_lo + n_pre; u < u_hi; ++u) {
                 const int tile = u / p.KB, kb = u - tile * p.KB;
                 br::mbar_wait(&empty_bar[s], ph ^ 1);
                 uint8_t* sa = smem + s * L::STAGE;
@@ -281,65 +264,14 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                 if (++s == L::NSTAGE) { s = 0; ph ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = br::make_idesc_bf16(BM, BNX);
-            if constexpr (PARK) {
-                for (int i = 0; i < n_park; ++i) {                                   // parking phase (before the dependency resolves)
-                    const int st = i % L::NSTAGE, use = i / L::NSTAGE;
-                    br::mbar_wait(&pfull_bar[st], use & 1);
-                    br::tc_fence_after();
-                    const uint64_t adesc = br::make_sw128_kmajor_desc(br::smem_u32(smem + st * L::STAGE));
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) br::tc_cp_128x256b(tmem_park + i * (BK / 2) + k * 8, adesc + 2 * k);
-                    br::tc_commit(&pempty_bar[st]);
-                }
-            }
-            int s = 0; uint32_t ph = 0; int as = 0; uint32_t aph = 0;
-            int u = u_lo;
-            bool xp_ready = false;
-            while (u < u_hi) {
-                const int tile = u / p.KB;
-                const int seg_end = min(u_hi, (tile + 1) * p.KB);
-                br::mbar_wait(&tempty_bar[as], aph ^ 1);
-                br::tc_fence_after();
-                const uint32_t tmem_d = tmem_base + as * BNX;
-                for (int i = 0; u < seg_end; ++u, ++i) {
-                    if constexpr (PARK) {
-                        if (u - u_lo < n_park) {                                     // weight tile in tensor memory, activation tile in xp
-                            if (!xp_ready) { br::mbar_wait(xp_bar, 0); br::tc_fence_after(); xp_ready = true; }
-                            const int j = u - u_lo;
-                            const uint64_t bdesc = br::make_sw128_kmajor_desc(br::smem_u32(xp + j * L::B_BYTES));
-#pragma unroll
-                            for (int k = 0; k < BK / 16; ++k)
-                                br::tc_mma_bf16_ts(tmem_d, tmem_park + j * (BK / 2) + k * 8, bdesc + 2 * k, idesc, (i | k) != 0);
-                            continue;
-                        }
-                    }
-                    br::mbar_wait(&full_bar[s], ph);
-                    if (u == u_hi - 1 && p.gate_counter && p.gate_signal)          // every weight tile of this CTA is on chip
-                        asm volatile("red.relaxed.gpu.global.add.s32 [%0], 1;" ::"l"(p.gate_counter) : "memory");
-                    br::tc_fence_after();
-                    const uint32_t sa = br::smem_u32(smem + s * L::STAGE);
-                    const uint64_t adesc = br::make_sw128_kmajor_desc(sa);
-                    const uint64_t bdesc = br::make_sw128_kmajor_desc(sa + L::A_BYTES);
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) br::tc_mma_bf16(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (i | k) != 0);
-                    br::tc_commit(&empty_bar[s]);
-                    if (++s == L::NSTAGE) { s = 0; ph ^= 1; }
-                }
-                br::tc_commit(&tfull_bar[as]);
-                if (++as == 2) { as = 0; aph ^= 1; }
-            }
-        }
     } else {
         const int lane_grp = warp & 3;
-        const int et = threadIdx.x - 64;                      // 0..127 within the epilogue group
-        SKSTAMP(2);                                           // TMEM allocated, barriers initialised
-        br::grid_dep_wait();                                  // everything below touches data shared with earlier kernels
+        const int et = threadIdx.x;                               // 0..127 within the consumer warpgroup
+        SKSTAMP(2);                                               // barriers initialised
+        br::grid_dep_wait();                                      // everything below touches data shared with earlier kernels
         SKSTAMP(1);
         compute_row_rstd(p, et, s_rs, s_rs + 32);
-        int as = 0; uint32_t aph = 0;
+        int s = 0; uint32_t ph = 0;
         int u = u_lo;
         while (u < u_hi) {
             const int tile = u / p.KB;
@@ -349,33 +281,10 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
             const int part_row = tile * 4 + lane_grp;
             float res[RM];
             load_residual<RM>(p, f, res);                        // in flight while the accumulator is still being produced
-            br::mbar_wait(&tfull_bar[as], aph);
-            if (u == u_lo) SKSTAMP(3);
-            br::tc_fence_after();
-            const uint32_t taddr = tmem_base + as * BNX + ((uint32_t)(lane_grp * 32) << 16);
             float v[RM];
-            if constexpr (RM == 8) {
-                uint32_t r[8];
-                __syncwarp();
-                tmem_ld_32x8(taddr, r);
-                br::tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-            } else {
-#pragma unroll
-                for (int c = 0; c < RM; c += 16) {
-                    uint32_t r[16];
-                    __syncwarp();
-                    tmem_ld_32x16(taddr + c, r);
-                    br::tmem_ld_wait();
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) v[c + i] = __uint_as_float(r[i]);
-                }
-            }
-            br::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) br::mbar_arrive(&tempty_bar[as]);   // accumulator drained into registers
-            if (++as == 2) { as = 0; aph ^= 1; }
+            mma_tile<BNX, RM>(smem, full_bar, empty_bar, s, ph, seg_end - u, (seg_end == u_hi && p.gate_counter && p.gate_signal) ? p.gate_counter : nullptr,
+                              s_tr, v);
+            if (u == u_lo) SKSTAMP(3);
             if (whole) {
                 apply_epilogue<RM>(p, f, lane, v, res, s_rs, part_row);
             } else {
@@ -388,7 +297,7 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                 const int first_c = (tile * p.KB) / p.chunk, last_c = ((tile + 1) * p.KB - 1) / p.chunk;
                 if ((int)blockIdx.x != first_c) {
                     float* mine = p.scratch + ((long long)blockIdx.x * 2 * BNX) * BM + lane_grp * 32 + lane;   // slot 0: the CTA's first tile
-#pragma unroll
+    #pragma unroll
                     for (int r = 0; r < RM; ++r)
                         if (r < p.R) __stcg(mine + r * BM, v[r]);
                     __syncwarp();
@@ -404,19 +313,19 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                     asm volatile("bar.sync 1, 128;" ::: "memory");
                     SKSTAMP(4);
                     for (int c0 = first_c + 1; c0 <= last_c; c0 += 8) {          // 8 contributors x 8 rows of loads in flight
-#pragma unroll
+    #pragma unroll
                         for (int r0 = 0; r0 < RM; r0 += 8) {
                             if (r0 >= p.R) break;                                // warp-uniform
                             float t[8][8];
-#pragma unroll
+    #pragma unroll
                             for (int j = 0; j < 8; ++j) {
                                 const float* src = p.scratch + ((long long)(c0 + j) * 2 * BNX) * BM + lane_grp * 32 + lane;
-#pragma unroll
+    #pragma unroll
                                 for (int r = 0; r < 8; ++r) t[j][r] = (c0 + j <= last_c && r0 + r < p.R) ? __ldcg(src + (r0 + r) * BM) : 0.f;
                             }
-#pragma unroll
+    #pragma unroll
                             for (int j = 0; j < 8; ++j)
-#pragma unroll
+    #pragma unroll
                                 for (int r = 0; r < 8; ++r) v[r0 + r] += t[j][r];            // ascending CTA order: deterministic
                         }
                     }
@@ -429,18 +338,12 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
         }
         SKSTAMP(7);
     }
-    br::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        br::tc_fence_after();
-        br::tmem_dealloc(tmem_base, L::TMEM_COLS);
-    }
 }
 
-template <int BNX, int RM, bool PARK>
+template <int BNX, int RM>
 int launch(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& tp, const SkParams& p, int grid, cudaStream_t st) {
-    using L = SL<BNX, PARK>;
-    auto kern = skinny_tc5_kernel<BNX, RM, PARK>;
+    using L = SL<BNX>;
+    auto kern = skinny_tc5_kernel<BNX, RM>;
     static bool done = false;
     if (!done) {
         BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
@@ -459,7 +362,7 @@ int launch(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& tp, 
 // producer thread loads the activation tiles and is the only one that waits for "phase inputs ready".
 // ================================================================================================================
 constexpr int CHAIN_MAX = 4;
-constexpr int CHAIN_THREADS = 224;           // warp 0: W producer, 1: MMA, 2-5: epilogue, 6: X producer
+constexpr int CHAIN_THREADS = 192;           // warps 0-3: wgmma + epilogue, 4: W producer, 5: X producer
 
 struct ChainPhase { CUtensorMap tmW; CUtensorMap tmX; SkParams p; };
 struct ChainParams { ChainPhase ph[CHAIN_MAX]; int n_phases; int* gbar; long long* dbg; };
@@ -468,15 +371,13 @@ __device__ __forceinline__ long long gtime() { long long t; asm volatile("mov.u6
 
 template <int BNX>
 __global__ void __launch_bounds__(CHAIN_THREADS, 1) skinny_chain_kernel(const __grid_constant__ ChainParams cp) {
-    using L = SL<BNX, false>;
+    using L = SL<BNX>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::TILE_BYTES);
+    float* s_tr = reinterpret_cast<float*>(smem + L::TILE_BYTES);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::TILE_BYTES + L::TR_BYTES);
     uint64_t* empty_bar = full_bar + L::NSTAGE;
-    uint64_t* tfull_bar = empty_bar + L::NSTAGE;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-    int* s_flag = reinterpret_cast<int*>(tmem_slot + 1);
+    int* s_flag = reinterpret_cast<int*>(empty_bar + L::NSTAGE);
     volatile int* s_ready = reinterpret_cast<volatile int*>(s_flag + 1);      // number of grid barriers this CTA has passed
     float* s_rs = reinterpret_cast<float*>(s_flag + 2);
 
@@ -484,23 +385,17 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) skinny_chain_kernel(const __
     const int nph = cp.n_phases;
 
     br::launch_dependents();
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         for (int i = 0; i < nph; ++i) { br::tma_prefetch_desc(&cp.ph[i].tmW); br::tma_prefetch_desc(&cp.ph[i].tmX); }
+        // full: the W producer's expect_tx covers both halves of a stage (the X producer's load completes the same count);
+        // empty: released by the consumer warpgroup, awaited by both producers
         for (int s = 0; s < L::NSTAGE; ++s) { br::mbar_init(&full_bar[s], 1); br::mbar_init(&empty_bar[s], 1); }
-        for (int s = 0; s < 2; ++s) { br::mbar_init(&tfull_bar[s], 1); br::mbar_init(&tempty_bar[s], 4); }
         br::mbar_fence_init();
         *s_ready = 0;
     }
-    if (warp == 1) {
-        br::tmem_alloc(tmem_slot, 2 * BNX < 32 ? 32 : 2 * BNX);
-        br::tmem_relinquish();
-    }
-    br::tc_fence_before();
     __syncthreads();
-    br::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 4) {
         // ---------------- weight producer: never waits for other kernels or phases (weights are constant) ----------------
         if (lane == 0) {
             int s = 0; uint32_t ph = 0;
@@ -516,7 +411,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) skinny_chain_kernel(const __
                 }
             }
         }
-    } else if (warp == 6) {
+    } else if (warp == 5) {
         // ---------------- activation producer: gated by "inputs of phase pi are complete" ----------------
         if (lane == 0) {
             br::grid_dep_wait();
@@ -533,44 +428,14 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) skinny_chain_kernel(const __
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = br::make_idesc_bf16(BM, BNX);
-            int s = 0; uint32_t ph = 0; int as = 0; uint32_t aph = 0;
-            for (int pi = 0; pi < nph; ++pi) {
-                const SkParams& p = cp.ph[pi].p;
-                const int u_lo = blockIdx.x * p.chunk, u_hi = min(p.units, u_lo + p.chunk);
-                int u = u_lo;
-                while (u < u_hi) {
-                    const int tile = u / p.KB;
-                    const int seg_end = min(u_hi, (tile + 1) * p.KB);
-                    br::mbar_wait(&tempty_bar[as], aph ^ 1);
-                    br::tc_fence_after();
-                    const uint32_t tmem_d = tmem_base + as * BNX;
-                    for (int i = 0; u < seg_end; ++u, ++i) {
-                        br::mbar_wait(&full_bar[s], ph);
-                        br::tc_fence_after();
-                        const uint32_t sa = br::smem_u32(smem + s * L::STAGE);
-                        const uint64_t adesc = br::make_sw128_kmajor_desc(sa);
-                        const uint64_t bdesc = br::make_sw128_kmajor_desc(sa + L::A_BYTES);
-#pragma unroll
-                        for (int k = 0; k < BK / 16; ++k) br::tc_mma_bf16(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (i | k) != 0);
-                        br::tc_commit(&empty_bar[s]);
-                        if (++s == L::NSTAGE) { s = 0; ph ^= 1; }
-                    }
-                    br::tc_commit(&tfull_bar[as]);
-                    if (++as == 2) { as = 0; aph ^= 1; }
-                }
-            }
-        }
     } else {
-        // ---------------- epilogue warps 2..5 ----------------
+        // ---------------- consumer warpgroup (warps 0..3): wgmma + epilogue ----------------
         const int lane_grp = warp & 3;
-        const int et = threadIdx.x - 64;
+        const int et = threadIdx.x;
         CSTAMP(0);
         br::grid_dep_wait();
         CSTAMP(1);
-        int as = 0; uint32_t aph = 0;
+        int s = 0; uint32_t ph = 0;
         for (int pi = 0; pi < nph; ++pi) {
             const SkParams& p = cp.ph[pi].p;
             const int u_lo = blockIdx.x * p.chunk, u_hi = min(p.units, u_lo + p.chunk);
@@ -581,24 +446,9 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) skinny_chain_kernel(const __
                 const int tile = u / p.KB;
                 const int seg_end = min(u_hi, (tile + 1) * p.KB);
                 const bool whole = (u == tile * p.KB) && (seg_end == (tile + 1) * p.KB);
-                br::mbar_wait(&tfull_bar[as], aph);
-                if (u == u_lo) CSTAMP(3 + pi * 6);
-                br::tc_fence_after();
-                const uint32_t taddr = tmem_base + as * BNX + ((uint32_t)(lane_grp * 32) << 16);
                 float v[BNX];
-#pragma unroll
-                for (int c = 0; c < BNX; c += 16) {
-                    uint32_t r[16];
-                    __syncwarp();
-                    tmem_ld_32x16(taddr + c, r);
-                    br::tmem_ld_wait();
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) v[c + i] = __uint_as_float(r[i]);
-                }
-                br::tc_fence_before();
-                __syncwarp();
-                if (lane == 0) br::mbar_arrive(&tempty_bar[as]);
-                if (++as == 2) { as = 0; aph ^= 1; }
+                mma_tile<BNX, BNX>(smem, full_bar, empty_bar, s, ph, seg_end - u, nullptr, s_tr, v);
+                if (u == u_lo) CSTAMP(3 + pi * 6);
                 const int f = tile * BM + lane_grp * 32 + lane;
                 const int part_row = tile * 4 + lane_grp;
                 float res[BNX];
@@ -664,17 +514,11 @@ __global__ void __launch_bounds__(CHAIN_THREADS, 1) skinny_chain_kernel(const __
             if (atomicAdd(cp.gbar + 1, 1) == (int)gridDim.x - 1) { cp.gbar[0] = 0; cp.gbar[1] = 0; __threadfence(); }
         }
     }
-    br::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        br::tc_fence_after();
-        br::tmem_dealloc(tmem_base, 2 * BNX < 32 ? 32 : 2 * BNX);
-    }
 }
 
 template <int BNX>
 int launch_chain(const ChainParams& cp, int grid, cudaStream_t st) {
-    using L = SL<BNX, false>;
+    using L = SL<BNX>;
     auto kern = skinny_chain_kernel<BNX>;
     static bool done = false;
     if (!done) { BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL)); done = true; }
@@ -765,19 +609,13 @@ int br_skinny_gemm_gated(const void* X, int64_t ldx, const void* W, int64_t ldw,
         p.pf_on = 1;
     }
     cudaStream_t st = (cudaStream_t)stream;
-    // BR_SKINNY_PARK=1: also buffer weight tiles in tensor memory before the dependency resolves (A/B switch until it is the measured default)
-    static const bool park = getenv("BR_SKINNY_PARK") && atoi(getenv("BR_SKINNY_PARK")) != 0;
-    if (park) {
-        if (R <= 8) return launch<16, 8, true>(tw, tx, tp, p, grid, st);
-        return BNX == 16 ? launch<16, 16, true>(tw, tx, tp, p, grid, st) : launch<32, 32, true>(tw, tx, tp, p, grid, st);
-    }
-    if (R <= 8) return launch<16, 8, false>(tw, tx, tp, p, grid, st);
-    return BNX == 16 ? launch<16, 16, false>(tw, tx, tp, p, grid, st) : launch<32, 32, false>(tw, tx, tp, p, grid, st);
+    if (R <= 8) return launch<16, 8>(tw, tx, tp, p, grid, st);
+    return BNX == 16 ? launch<16, 16>(tw, tx, tp, p, grid, st) : launch<32, 32>(tw, tx, tp, p, grid, st);
 }
 
 
 /* profiling aid: [n_launches, 160, 8] int64 %globaltimer stamps of the next br_skinny_gemm launches (NULL disables):
- * 0 kernel entry, 1 dependency wait passed, 2 prologue done (TMEM allocated, barriers initialised), 3 first accumulator, 4 last partial published, 5 reduction loads done,
+ * 0 kernel entry, 1 dependency wait passed, 2 prologue done (barriers initialised), 3 first accumulator, 4 last partial published, 5 reduction loads done,
  * 6 reducer epilogue done, 7 CTA done */
 int br_skinny_debug(long long* buf) { g_sk_dbg = buf; g_sk_dbg_slot = 0; return BR_OK; }
 

@@ -1,24 +1,25 @@
-// tcgen05 / TMEM / TMA GEMM for sm_100a:  D[M,N] = alpha * (A[M,K] . B[N,K]^T  (+ A2[M,K2] . B2[N,K2]^T)) (+bias)(+residual)
+// wgmma / TMA GEMM for sm_90a:  D[M,N] = alpha * (A[M,K] . B[N,K]^T  (+ A2[M,K2] . B2[N,K2]^T)) (+bias)(+residual)
 //
 // Replaces every nn.Linear / lm_head matmul the reference reaches through HF (SURVEY.md §2.3 K1,K2,K5,K6,K12):
-// both operands are K-major (nn.Linear weight layout [out, in]), bf16 in, fp32 accumulate in TMEM.
+// both operands are K-major (nn.Linear weight layout [out, in]), bf16 in, fp32 accumulate in registers.
 //
-// Structure (one persistent CTA per SM, 192 threads):
-//   warp 0      TMA producer   : cp.async.bulk.tensor 2-D, 128B-swizzled 128x64 (A) and BNx64 (B) tiles, NSTAGE ring
-//   warp 1      MMA issuer     : one lane issues tcgen05.mma.cta_group::1.kind::f16 (UMMA 128 x BN x 16), accumulators
-//                                double-buffered in TMEM (2 x BN fp32 columns) so the epilogue of tile i overlaps the
-//                                main loop of tile i+1; tcgen05.commit releases smem stages / publishes accumulators
-//   warps 2..5  epilogue       : tcgen05.ld 32x32b.x32 (thread <-> accumulator row), fused epilogue, vectorised stores
+// Structure (one persistent CTA per SM, 288 threads):
+//   warp 8      TMA producer   : cp.async.bulk.tensor 2-D, 128B-swizzled 128x64 (A) and 128x64 (B) tiles, NSTAGE ring
+//   warps 0..7  two consumer warpgroups: each issues wgmma.mma_async m64n128k16 for its 64 rows of the 128 x 128 tile (one
+//                                wgmma group kept in flight; a stage goes back to the producer as soon as its products retire),
+//                                then runs the fused epilogue straight from the register fragment
 // Epilogue modes: plain (+bias, +residual, gated-SiLU on interleaved column pairs, fp32/bf16 out, row scatter),
 // online log-sum-exp partials + target-logit gather (lm_head; logits never reach HBM), and softmax-gradient tiles.
 #include "br_common.cuh"
 #include "../../include/bioreason_b200.h"
+#include "wgmma.cuh"
 
 namespace {
 
 constexpr int BM = 128;
+constexpr int BN = 128;
 constexpr int BK = 64;
-constexpr int NTHREADS = 192;
+constexpr int NTHREADS = 288;
 
 enum { MODE_STD = 0, MODE_LSE = 1, MODE_DLOGITS = 2 };
 
@@ -41,21 +42,18 @@ struct GemmParams {
     int group_m;             // m-blocks per raster group (see tile_coords)
 };
 
-template <int BN>
 struct SmemLayout {
     static constexpr int A_BYTES = BM * BK * 2;
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int NSTAGE = (BN == 256) ? 4 : 6;
+    static constexpr int NSTAGE = 6;                        // 6 x 32 KB of the 227 KB a block may use
     static constexpr int TILE_BYTES = NSTAGE * STAGE_BYTES;
     static constexpr int TOTAL = TILE_BYTES + 256 + 1024;   // + barriers + alignment slack
 };
 
 __device__ __forceinline__ void tile_coords(int tile, int ntm, int ntn, int GROUP_M, int& mb, int& nb) {
     // grouped rasterisation: GROUP_M m-blocks x all n-blocks per group.  The group's A panel (GROUP_M x 128 x K, sized by the host to
-    // ~40 MB) stays L2-resident while every B panel streams past it once, so B is re-read from DRAM once per GROUP (with the fixed
-    // GROUP_M = 16 of round 1 the [18880 x 2560] x [19456 x 2560]^T gate/up GEMM re-read B 9 times: 1.08 GB of DRAM reads for 196 MB
-    // of operands).
+    // about a third of L2) stays L2-resident while every B panel streams past it once, so B is re-read from DRAM once per GROUP.
     int per_group = GROUP_M * ntn;
     int g = tile / per_group;
     int first_m = g * GROUP_M;
@@ -65,19 +63,18 @@ __device__ __forceinline__ void tile_coords(int tile, int ntm, int ntn, int GROU
     nb = r / gsize;
 }
 
-template <int BN, int MODE>
+__device__ __forceinline__ float rbf(float x) { return __bfloat162float(__float2bfloat16(x)); }
+
+template <int MODE>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
                 const GemmParams p) {
-    using L = SmemLayout<BN>;
+    using L = SmemLayout;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::TILE_BYTES);
     uint64_t* empty_bar = full_bar + L::NSTAGE;
-    uint64_t* tfull_bar = empty_bar + L::NSTAGE;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -86,24 +83,16 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     const int kb2 = (p.K2 + BK - 1) / BK;
     const int num_kb = kb1 + kb2;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         br::tma_prefetch_desc(&tmA);
         br::tma_prefetch_desc(&tmB);
         if (kb2) { br::tma_prefetch_desc(&tmA2); br::tma_prefetch_desc(&tmB2); }
-        for (int s = 0; s < L::NSTAGE; ++s) { br::mbar_init(&full_bar[s], 1); br::mbar_init(&empty_bar[s], 1); }
-        for (int s = 0; s < 2; ++s) { br::mbar_init(&tfull_bar[s], 1); br::mbar_init(&tempty_bar[s], 4); }
+        for (int s = 0; s < L::NSTAGE; ++s) { br::mbar_init(&full_bar[s], 1); br::mbar_init(&empty_bar[s], 2); }
         br::mbar_fence_init();
     }
-    if (warp == 1) {
-        br::tmem_alloc(tmem_slot, 2 * BN);
-        br::tmem_relinquish();
-    }
-    br::tc_fence_before();
     __syncthreads();
-    br::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ===================== TMA producer =====================
         if (lane == 0) {
             int s = 0; uint32_t ph = 0;
@@ -125,209 +114,149 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            constexpr uint32_t idesc = br::make_idesc_bf16(BM, BN);
-            int s = 0; uint32_t ph = 0; int as = 0; uint32_t aph = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                br::mbar_wait(&tempty_bar[as], aph ^ 1);
-                br::tc_fence_after();
-                const uint32_t tmem_d = tmem_base + as * BN;
-                for (int kb = 0; kb < num_kb; ++kb) {
-                    br::mbar_wait(&full_bar[s], ph);
-                    br::tc_fence_after();
-                    const uint32_t sa = br::smem_u32(smem + s * L::STAGE_BYTES);
-                    const uint64_t adesc = br::make_sw128_kmajor_desc(sa);
-                    const uint64_t bdesc = br::make_sw128_kmajor_desc(sa + L::A_BYTES);
+        return;
+    }
+    // ===================== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the 128 x BN tile =====================
+    const int wg = warp >> 2;
+    const int wt = threadIdx.x & 127;
+    int s = 0; uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int mb, nb; tile_coords(tile, p.n_tiles_m, p.n_tiles_n, p.group_m, mb, nb);
+        float acc[BN / 2];
 #pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        // advance 16 bf16 = 32 B along K inside the 128 B swizzle span: +2 in the (addr >> 4) field
-                        br::tc_mma_bf16(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0);
-                    }
-                    br::tc_commit(&empty_bar[s]);          // smem stage reusable once these MMAs retire
-                    if (++s == L::NSTAGE) { s = 0; ph ^= 1; }
-                }
-                br::tc_commit(&tfull_bar[as]);             // accumulator ready for the epilogue warps
-                if (++as == 2) { as = 0; aph ^= 1; }
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        int prev = 0;
+        for (int kb = 0; kb < num_kb; ++kb) {
+            br::mbar_wait(&full_bar[s], ph);
+            const uint32_t sa = br::smem_u32(smem + s * L::STAGE_BYTES);
+            const uint64_t adesc = br::wg_desc_k(sa + wg * 64 * 128);
+            const uint64_t bdesc = br::wg_desc_k(sa + L::A_BYTES);
+            br::wg_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) br::wgmma_ss<BN>(acc, adesc + 2 * k, bdesc + 2 * k, 1);
+            br::wg_commit();
+            if (kb > 0) {                                  // the previous stage's products have retired: hand it back
+                br::wg_wait<1>();
+                if (wt == 0) br::mbar_arrive(&empty_bar[prev]);
             }
+            prev = s;
+            if (++s == L::NSTAGE) { s = 0; ph ^= 1; }
         }
-    } else {
-        // ===================== epilogue (warps 2..5) =====================
-        const int lane_grp = warp & 3;                     // TMEM lane group this warp may access
-        int as = 0; uint32_t aph = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-            int mb, nb; tile_coords(tile, p.n_tiles_m, p.n_tiles_n, p.group_m, mb, nb);
-            br::mbar_wait(&tfull_bar[as], aph);
-            br::tc_fence_after();
-            const int row = mb * BM + lane_grp * 32 + lane;
-            const bool row_ok = row < p.M;
-            const uint32_t taddr = tmem_base + as * BN + ((uint32_t)(lane_grp * 32) << 16);
-            const int n0 = nb * BN;
+        br::wg_wait<0>();
+        br::wg_fence_operand(acc);
+        if (wt == 0) br::mbar_arrive(&empty_bar[prev]);
 
-            if constexpr (MODE == MODE_STD) {
-                long long orow = row;
-                if (p.row_map && row_ok) orow = p.row_map[row];
-                const bool store_ok = row_ok && orow >= 0;
-#pragma unroll 1
-                for (int c = 0; c < BN; c += 32) {
-                    if (n0 + c >= p.N) break;              // warp-uniform
-                    uint32_t r[32];
-                    __syncwarp();
-                    br::tmem_ld_32x32(taddr + c, r);
-                    br::tmem_ld_wait();
-                    if (!store_ok) continue;
-                    float v[32];
+        // ---- epilogue straight from the accumulator fragment: thread holds rows r0, r0 + 8 and column pairs 8i + 2 (lane % 4)
+        const int r0 = mb * BM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int n0 = nb * BN;
+        const int cq = 2 * (lane & 3);
+        if constexpr (MODE == MODE_STD) {
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]) * p.alpha;
-                    const int col = n0 + c;
-                    const int ncols = min(32, p.N - col);  // multiple of 8 (N % 8 == 0)
-                    if (p.bias) {
+            for (int hh = 0; hh < 2; ++hh) {
+                const int row = r0 + 8 * hh;
+                if (row >= p.M) continue;
+                const long long orow = p.row_map ? (long long)p.row_map[row] : (long long)row;
+                if (orow < 0) continue;
+                float v[BN / 4];
+#pragma unroll
+                for (int i = 0; i < BN / 8; ++i) {
+                    v[2 * i] = acc[4 * i + 2 * hh] * p.alpha;
+                    v[2 * i + 1] = acc[4 * i + 2 * hh + 1] * p.alpha;
+                    const int col = n0 + 8 * i + cq;
+                    if (p.bias && n0 + 8 * i < p.N) {
                         if (p.bias_f32) {
                             const float* b = reinterpret_cast<const float*>(p.bias) + col;
-#pragma unroll
-                            for (int i = 0; i < 32; ++i) if (i < ncols) v[i] += __ldg(b + i);
+                            v[2 * i] += __ldg(b); v[2 * i + 1] += __ldg(b + 1);
                         } else {
                             const bf16* b = reinterpret_cast<const bf16*>(p.bias) + col;
-#pragma unroll
-                            for (int i = 0; i < 32; ++i) if (i < ncols) v[i] += __bfloat162float(b[i]);
+                            v[2 * i] += __bfloat162float(b[0]); v[2 * i + 1] += __bfloat162float(b[1]);
                         }
                     }
-                    if (p.act == 1) {
+                }
+                if (p.act == 1) {
+#pragma unroll
+                    for (int j = 0; j < BN / 16; ++j) {
+                        if (n0 + 16 * j >= p.N) break;
                         if (p.aux) {
-                            uint4* a = reinterpret_cast<uint4*>(p.aux + orow * p.ld_aux + col);
-#pragma unroll
-                            for (int q = 0; q < 4; ++q)
-                                if (q * 8 < ncols)
-                                    a[q] = make_uint4(br::pack_bf16(v[q * 8 + 0], v[q * 8 + 1]), br::pack_bf16(v[q * 8 + 2], v[q * 8 + 3]),
-                                                      br::pack_bf16(v[q * 8 + 4], v[q * 8 + 5]), br::pack_bf16(v[q * 8 + 6], v[q * 8 + 7]));
+                            bf16* a = p.aux + orow * p.ld_aux + n0 + 16 * j + cq;
+                            *reinterpret_cast<uint32_t*>(a) = br::pack_bf16(v[4 * j], v[4 * j + 1]);
+                            *reinterpret_cast<uint32_t*>(a + 8) = br::pack_bf16(v[4 * j + 2], v[4 * j + 3]);
                         }
-                        float o[16];
+                        // columns come in blocks of 16 = 8 gate | 8 up (packing.py); HF computes act_fn(gate) in bf16 then multiplies:
+                        // round at the same places
+                        float o[2];
 #pragma unroll
-                        for (int i = 0; i < 16; ++i) {
-                            // columns come in blocks of 16 = 8 gate | 8 up (packing.py); HF computes act_fn(gate) in bf16
-                            // then multiplies: round at the same places
-                            const int gi = (i >> 3) * 16 + (i & 7);
-                            float g = __bfloat162float(__float2bfloat16(v[gi])), u = __bfloat162float(__float2bfloat16(v[gi + 8]));
-                            float sg = __bfloat162float(__float2bfloat16(g / (1.f + __expf(-g))));
-                            o[i] = sg * u;
+                        for (int e = 0; e < 2; ++e) {
+                            const float g = rbf(v[4 * j + e]), u = rbf(v[4 * j + 2 + e]);
+                            o[e] = rbf(g / (1.f + __expf(-g))) * u;
                         }
-                        bf16* d = reinterpret_cast<bf16*>(p.D) + orow * (long long)p.ldd + col / 2;
-                        uint4* d4 = reinterpret_cast<uint4*>(d);
-#pragma unroll
-                        for (int q = 0; q < 2; ++q)
-                            if (q * 16 < ncols)
-                                d4[q] = make_uint4(br::pack_bf16(o[q * 8 + 0], o[q * 8 + 1]), br::pack_bf16(o[q * 8 + 2], o[q * 8 + 3]),
-                                                   br::pack_bf16(o[q * 8 + 4], o[q * 8 + 5]), br::pack_bf16(o[q * 8 + 6], o[q * 8 + 7]));
-                        continue;
+                        bf16* d = reinterpret_cast<bf16*>(p.D) + orow * (long long)p.ldd + (n0 >> 1) + 8 * j + cq;
+                        *reinterpret_cast<uint32_t*>(d) = br::pack_bf16(o[0], o[1]);
                     }
+                    continue;
+                }
+#pragma unroll
+                for (int i = 0; i < BN / 8; ++i) {
+                    if (n0 + 8 * i >= p.N) break;
+                    const int col = n0 + 8 * i + cq;
+                    float x0 = v[2 * i], x1 = v[2 * i + 1];
                     if (p.residual) {
-                        const uint4* rp = reinterpret_cast<const uint4*>(p.residual + orow * p.ldr + col);
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) {
-                            if (q * 8 < ncols) {
-                                uint4 rr = __ldg(rp + q);
-                                float2 a = br::unpack_bf16(rr.x), b = br::unpack_bf16(rr.y), c2 = br::unpack_bf16(rr.z), d2 = br::unpack_bf16(rr.w);
-                                // nn.Linear output is rounded to bf16 before the residual add in HF
-                                v[q * 8 + 0] = __bfloat162float(__float2bfloat16(v[q * 8 + 0])) + a.x;
-                                v[q * 8 + 1] = __bfloat162float(__float2bfloat16(v[q * 8 + 1])) + a.y;
-                                v[q * 8 + 2] = __bfloat162float(__float2bfloat16(v[q * 8 + 2])) + b.x;
-                                v[q * 8 + 3] = __bfloat162float(__float2bfloat16(v[q * 8 + 3])) + b.y;
-                                v[q * 8 + 4] = __bfloat162float(__float2bfloat16(v[q * 8 + 4])) + c2.x;
-                                v[q * 8 + 5] = __bfloat162float(__float2bfloat16(v[q * 8 + 5])) + c2.y;
-                                v[q * 8 + 6] = __bfloat162float(__float2bfloat16(v[q * 8 + 6])) + d2.x;
-                                v[q * 8 + 7] = __bfloat162float(__float2bfloat16(v[q * 8 + 7])) + d2.y;
-                            }
-                        }
+                        // nn.Linear output is rounded to bf16 before the residual add in HF
+                        const float2 r = br::unpack_bf16(__ldg(reinterpret_cast<const unsigned int*>(p.residual + orow * p.ldr + col)));
+                        x0 = rbf(x0) + r.x; x1 = rbf(x1) + r.y;
                     }
-                    if (p.out_f32) {
-                        float4* d4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.D) + orow * (long long)p.ldd + col);
-#pragma unroll
-                        for (int q = 0; q < 8; ++q)
-                            if (q * 4 < ncols) d4[q] = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
-                    } else {
-                        uint4* d4 = reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(p.D) + orow * (long long)p.ldd + col);
-#pragma unroll
-                        for (int q = 0; q < 4; ++q)
-                            if (q * 8 < ncols)
-                                d4[q] = make_uint4(br::pack_bf16(v[q * 8 + 0], v[q * 8 + 1]), br::pack_bf16(v[q * 8 + 2], v[q * 8 + 3]),
-                                                   br::pack_bf16(v[q * 8 + 4], v[q * 8 + 5]), br::pack_bf16(v[q * 8 + 6], v[q * 8 + 7]));
-                    }
+                    if (p.out_f32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.D) + orow * (long long)p.ldd + col) = make_float2(x0, x1);
+                    else *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.D) + orow * (long long)p.ldd + col) = br::pack_bf16(x0, x1);
                 }
-            } else if constexpr (MODE == MODE_LSE) {
-                // per-row online max / sum-exp over this tile's columns + target-logit pick
-                float mx = -INFINITY, sm = 0.f;
+            }
+        } else if constexpr (MODE == MODE_LSE) {
+            // per-row max / sum-exp over this tile's columns (the four lanes of a quad share a row) + target-logit pick
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                const int row = r0 + 8 * hh;
+                const bool row_ok = row < p.M;
                 const int tgt = row_ok ? p.target[row] : -1;
-#pragma unroll 1
-                for (int c = 0; c < BN; c += 32) {
-                    if (n0 + c >= p.N) break;
-                    uint32_t r[32];
-                    __syncwarp();
-                    br::tmem_ld_32x32(taddr + c, r);
-                    br::tmem_ld_wait();
-                    const int col = n0 + c;
-                    const int ncols = min(32, p.N - col);
-                    float cm = -INFINITY;
+                float mx = -INFINITY;
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) if (i < ncols) cm = fmaxf(cm, __uint_as_float(r[i]) * p.alpha);
-                    const float nm = fmaxf(mx, cm);
-                    float acc = 0.f;
+                for (int i = 0; i < BN / 8; ++i)
+                    if (n0 + 8 * i < p.N) mx = fmaxf(mx, fmaxf(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]) * p.alpha);
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                float sm = 0.f;
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) if (i < ncols) acc += __expf(__uint_as_float(r[i]) * p.alpha - nm);
-                    sm = sm * __expf(mx - nm) + acc;
-                    mx = nm;
-                    if (tgt >= col && tgt < col + ncols) {
-                        float t = 0.f;
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) if (col + i == tgt) t = __uint_as_float(r[i]) * p.alpha;
-                        p.tgt_logit[row] = t;
-                    }
+                for (int i = 0; i < BN / 8; ++i) {
+                    if (n0 + 8 * i >= p.N) continue;
+                    const int col = n0 + 8 * i + cq;
+                    const float x0 = acc[4 * i + 2 * hh] * p.alpha, x1 = acc[4 * i + 2 * hh + 1] * p.alpha;
+                    sm += __expf(x0 - mx) + __expf(x1 - mx);
+                    if (col == tgt) p.tgt_logit[row] = x0;
+                    if (col + 1 == tgt) p.tgt_logit[row] = x1;
                 }
-                if (row_ok) {
+                sm += __shfl_xor_sync(0xffffffffu, sm, 1);
+                sm += __shfl_xor_sync(0xffffffffu, sm, 2);
+                if (row_ok && (lane & 3) == 0) {
                     p.pmax[(long long)row * p.n_tiles_n + nb] = mx;
                     p.psum[(long long)row * p.n_tiles_n + nb] = sm;
                 }
-            } else {
-                // dlogits[m, n] = gscale[m] * (onehot(target[m])[n] - exp(logit - lse[m]))   (bf16 out)
-                const int tgt = row_ok ? p.target[row] : -1;
-                const float lse = row_ok ? p.lse[row] : 0.f;
-                const float gs = row_ok ? p.gscale[row] : 0.f;
-#pragma unroll 1
-                for (int c = 0; c < BN; c += 32) {
-                    if (n0 + c >= p.N) break;
-                    uint32_t r[32];
-                    __syncwarp();
-                    br::tmem_ld_32x32(taddr + c, r);
-                    br::tmem_ld_wait();
-                    if (!row_ok) continue;
-                    const int col = n0 + c;
-                    const int ncols = min(32, p.N - col);
-                    float v[32];
+            }
+        } else {
+            // dlogits[m, n] = gscale[m] * (onehot(target[m])[n] - exp(logit - lse[m]))   (bf16 out)
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        float pr = __expf(__uint_as_float(r[i]) * p.alpha - lse);
-                        v[i] = gs * (((col + i) == tgt ? 1.f : 0.f) - pr);
-                    }
-                    uint4* d4 = reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(p.D) + (long long)row * p.ldd + col);
+            for (int hh = 0; hh < 2; ++hh) {
+                const int row = r0 + 8 * hh;
+                if (row >= p.M) continue;
+                const int tgt = p.target[row];
+                const float lse = p.lse[row], gs = p.gscale[row];
 #pragma unroll
-                    for (int q = 0; q < 4; ++q)
-                        if (q * 8 < ncols)
-                            d4[q] = make_uint4(br::pack_bf16(v[q * 8 + 0], v[q * 8 + 1]), br::pack_bf16(v[q * 8 + 2], v[q * 8 + 3]),
-                                               br::pack_bf16(v[q * 8 + 4], v[q * 8 + 5]), br::pack_bf16(v[q * 8 + 6], v[q * 8 + 7]));
+                for (int i = 0; i < BN / 8; ++i) {
+                    if (n0 + 8 * i >= p.N) break;
+                    const int col = n0 + 8 * i + cq;
+                    const float d0 = gs * ((col == tgt ? 1.f : 0.f) - __expf(acc[4 * i + 2 * hh] * p.alpha - lse));
+                    const float d1 = gs * ((col + 1 == tgt ? 1.f : 0.f) - __expf(acc[4 * i + 2 * hh + 1] * p.alpha - lse));
+                    *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.D) + (long long)row * p.ldd + col) = br::pack_bf16(d0, d1);
                 }
             }
-            br::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) br::mbar_arrive(&tempty_bar[as]);
-            if (++as == 2) { as = 0; aph ^= 1; }
         }
-    }
-
-    br::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        br::tc_fence_after();
-        br::tmem_dealloc(tmem_base, 2 * BN);
     }
 }
 
@@ -364,18 +293,17 @@ PFN_encodeTiled get_encode() {
     return fn;
 }
 
-template <int BN, int MODE>
+template <int MODE>
 int launch(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& a2, const CUtensorMap& b2, const GemmParams& p, cudaStream_t st) {
-    using L = SmemLayout<BN>;
-    auto kern = gemm_tc5_kernel<BN, MODE>;
+    auto kern = gemm_tc5_kernel<MODE>;
     static bool attr_set = false;
     if (!attr_set) {
-        BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
+        BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemLayout::TOTAL));
         attr_set = true;
     }
     int tiles = p.n_tiles_m * p.n_tiles_n;
     int grid = tiles < br_num_sms() ? tiles : br_num_sms();
-    kern<<<grid, NTHREADS, L::TOTAL, st>>>(a, b, a2, b2, p);
+    kern<<<grid, NTHREADS, SmemLayout::TOTAL, st>>>(a, b, a2, b2, p);
     BR_CHECK_LAUNCH();
     return BR_OK;
 }
@@ -385,13 +313,12 @@ int run_gemm(int mode, const void* A, int64_t lda, const void* B, int64_t ldb, i
     BR_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
     BR_CHECK_ARG(N % 8 == 0 && K % 8 == 0 && lda % 8 == 0 && ldb % 8 == 0, "gemm: N, K, lda, ldb must be multiples of 8");
     BR_CHECK_ARG(((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0), "gemm: operands must be 16-byte aligned");
-    const int BN = (N <= 128 || (long long)((M + 127) / 128) * ((N + 255) / 256) < br_num_sms()) ? 128 : 256;
     p.M = M; p.N = N; p.K = K; p.K2 = (A2 && B2) ? K2 : 0;
     p.n_tiles_m = (M + BM - 1) / BM;
     p.n_tiles_n = (N + BN - 1) / BN;
-    {   // A panel of one raster group ~ 40 MB of the 126 MB L2 (the concurrently streaming B panels and the outputs need the rest)
+    {   // A panel of one raster group ~ 16 MB of the 50 MB L2 (the concurrently streaming B panels and the outputs need the rest)
         const long long a_block = (long long)BM * (K + p.K2) * 2;
-        long long g = (40ll << 20) / (a_block > 0 ? a_block : 1);
+        long long g = (16ll << 20) / (a_block > 0 ? a_block : 1);
         if (g < 8) g = 8;
         if (g > p.n_tiles_m) g = p.n_tiles_m;
         p.group_m = (int)g;
@@ -405,17 +332,9 @@ int run_gemm(int mode, const void* A, int64_t lda, const void* B, int64_t ldb, i
         if ((rc = br_make_tmap_2d_bf16(&ta2, A2, M, K2, lda2, BM))) return rc;
         if ((rc = br_make_tmap_2d_bf16(&tb2, B2, N, K2, ldb2, BN))) return rc;
     } else { ta2 = ta; tb2 = tb; }
-#define BR_LAUNCH(bn, md) return launch<bn, md>(ta, tb, ta2, tb2, p, st)
-    if (BN == 128) {
-        if (mode == MODE_STD) BR_LAUNCH(128, MODE_STD);
-        if (mode == MODE_LSE) BR_LAUNCH(128, MODE_LSE);
-        BR_LAUNCH(128, MODE_DLOGITS);
-    } else {
-        if (mode == MODE_STD) BR_LAUNCH(256, MODE_STD);
-        if (mode == MODE_LSE) BR_LAUNCH(256, MODE_LSE);
-        BR_LAUNCH(256, MODE_DLOGITS);
-    }
-#undef BR_LAUNCH
+    if (mode == MODE_STD) return launch<MODE_STD>(ta, tb, ta2, tb2, p, st);
+    if (mode == MODE_LSE) return launch<MODE_LSE>(ta, tb, ta2, tb2, p, st);
+    return launch<MODE_DLOGITS>(ta, tb, ta2, tb2, p, st);
 }
 
 }  // namespace
@@ -459,7 +378,7 @@ int br_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ldb, void* D
 }
 
 int64_t br_lmhead_workspace_bytes(int M, int V) {
-    int nt = (V + 127) / 128;   // worst case (BN = 128)
+    int nt = (V + 127) / 128;   // BN = 128
     return (int64_t)M * nt * 2 * sizeof(float) + (int64_t)M * sizeof(float);
 }
 

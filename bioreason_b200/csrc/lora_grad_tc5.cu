@@ -1,18 +1,19 @@
-// LoRA weight gradients on tcgen05:  out (+)= big[M, P]^T . small[M, N]   (contraction over the M tokens; fp32 out, N <= 128).
+// LoRA weight gradients on wgmma (sm_90a):  out (+)= big[M, P]^T . small[M, N]   (contraction over the M tokens; fp32 out, N <= 128).
 //
 // Autograd of the adapters the reference trains with peft (reason.py:362-394): dB = dy^T t and dA = u^T x (SURVEY.md §2.3 K12).
-// Both operands are read exactly as the forward/backward left them -- token-major [M, features] -- as MN-MAJOR tcgen05 operands
+// Both operands are read exactly as the forward/backward left them -- token-major [M, features] -- as MN-MAJOR wgmma operands
 // (the TMA box [64 tokens x 64 features] is one swizzle atom column; no transposed copies).  One launch covers a whole fused linear:
-// the full [P, N] product of e.g. dqkv^T (6144 features) with t_qkv (3r columns) is formed in TMEM and the epilogue writes only the
+// the full [P, N] product of e.g. dqkv^T (6144 features) with t_qkv (3r columns) is formed in registers and the epilogue writes only the
 // block each adapter owns (q rows x its r columns, ...), so 14 launches per decoder layer become 8.
-// Split-K over the token dimension fills the 148 SMs for narrow outputs; partial tiles are exchanged through a workspace and summed
+// Split-K over the token dimension fills the SMs for narrow outputs; partial tiles are exchanged through a workspace and summed
 // by the split-0 CTA in ascending split order (release/acquire counter, no floating-point atomics): gradients are bit-reproducible.
 #include "br_common.cuh"
 #include "../../include/bioreason_b200.h"
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int BM = 128, BKT = 64, NTHREADS = 192, NSTAGE = 4;
+constexpr int BM = 128, BKT = 64, NTHREADS = 160, NSTAGE = 4;   // warps 0..3: wgmma + epilogue, warp 4: TMA
 constexpr int A_BYTES = 2 * 64 * 128;          // two [64 tokens x 64 features] blocks
 constexpr int B_BLK = 64 * 128;
 
@@ -30,14 +31,12 @@ struct TnParams {
 template <int NPAD>
 __global__ void __launch_bounds__(NTHREADS, 1)
 tn_gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TnParams p) {
-    constexpr int NBB = (NPAD + 63) / 64;
+    constexpr int NBB = NPAD / 64;
     constexpr int STAGE = A_BYTES + NBB * B_BLK;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + NSTAGE * STAGE);
     uint64_t* empty_bar = full_bar + NSTAGE;
-    uint64_t* acc_bar = empty_bar + NSTAGE;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_bar + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile = blockIdx.x / p.splits, split = blockIdx.x % p.splits;
@@ -45,19 +44,14 @@ tn_gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     const int kb_lo = split * kb_per, kb_hi = min(p.kb_total, kb_lo + kb_per);
     const int n_kb = max(0, kb_hi - kb_lo);
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         br::tma_prefetch_desc(&tmA); br::tma_prefetch_desc(&tmB);
         for (int s = 0; s < NSTAGE; ++s) { br::mbar_init(&full_bar[s], 1); br::mbar_init(&empty_bar[s], 1); }
-        br::mbar_init(acc_bar, 1);
         br::mbar_fence_init();
     }
-    if (warp == 1) { br::tmem_alloc(tmem_slot, NPAD <= 32 ? 32 : (NPAD <= 64 ? 64 : 128)); br::tmem_relinquish(); }
-    br::tc_fence_before();
     __syncthreads();
-    br::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 4) {
         if (lane == 0) {
             int s = 0; uint32_t ph = 0;
             for (int kb = kb_lo; kb < kb_hi; ++kb) {
@@ -71,51 +65,56 @@ tn_gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
                 if (++s == NSTAGE) { s = 0; ph ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0 && n_kb > 0) {
-            constexpr uint32_t idesc = br::make_idesc_bf16_major(BM, NPAD, 1, 1);      // both operands MN-major
-            int s = 0; uint32_t ph = 0;
-            for (int i = 0; i < n_kb; ++i) {
-                br::mbar_wait(&full_bar[s], ph);
-                br::tc_fence_after();
-                const uint32_t sa = br::smem_u32(smem + s * STAGE);
+        return;
+    }
+    // ---- one consumer warpgroup: two m64 products (features 0..63 and 64..127 of the tile), both operands MN-major
+    const int et = threadIdx.x;                                          // 0..127
+    const int row = et;                                                  // product row of this thread in the epilogue
+    const int prow = tile * BM + row;                                    // row of the product = feature index of `big`
+    float v[NPAD];
+    if (n_kb > 0) {
+        float acc0[NPAD / 2], acc1[NPAD / 2];
 #pragma unroll
-                for (int kk = 0; kk < BKT / 16; ++kk) {
-                    // 16 tokens = 2 groups of 8 rows (SBO 1024 B); 64-feature blocks are 8192 B apart (LBO)
-                    const uint64_t ad = br::make_sw128_mnmajor_desc(sa + kk * 2048, 64 * 128, 1024);
-                    const uint64_t bd = br::make_sw128_mnmajor_desc(sa + A_BYTES + kk * 2048, B_BLK, 1024);
-                    br::tc_mma_bf16(tmem_base, ad, bd, idesc, (i | kk) != 0);
+        for (int i = 0; i < NPAD / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+        int s = 0; uint32_t ph = 0;
+        for (int i = 0; i < n_kb; ++i) {
+            br::mbar_wait(&full_bar[s], ph);
+            const uint32_t sa = br::smem_u32(smem + s * STAGE);
+            br::wg_fence();
+#pragma unroll
+            for (int kk = 0; kk < BKT / 16; ++kk) {
+                // 16 tokens = 2 groups of 8 rows (SBO 1024 B); 64-wide feature / column blocks are 8192 B apart (LBO)
+                const uint64_t bd = br::wg_desc_mn(sa + A_BYTES + kk * 2048, B_BLK, 1024);
+                br::wgmma_ss<NPAD, 1, 1>(acc0, br::wg_desc_mn(sa + kk * 2048, 64 * 128, 1024), bd, 1);
+                br::wgmma_ss<NPAD, 1, 1>(acc1, br::wg_desc_mn(sa + 64 * 128 + kk * 2048, 64 * 128, 1024), bd, 1);
+            }
+            br::wg_commit();
+            br::wg_wait<0>();
+            if (et == 0) br::mbar_arrive(&empty_bar[s]);
+            if (++s == NSTAGE) { s = 0; ph ^= 1; }
+        }
+        br::wg_fence_operand(acc0);
+        br::wg_fence_operand(acc1);
+        // every stage has been consumed and no load is in flight: the ring becomes the transpose buffer (one product row per thread)
+        float* s_t = reinterpret_cast<float*>(smem);
+        const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+        for (int i = 0; i < NPAD / 8; ++i)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    s_t[(fr + 8 * hh) * (NPAD + 1) + 8 * i + fc + e] = acc0[4 * i + 2 * hh + e];
+                    s_t[(64 + fr + 8 * hh) * (NPAD + 1) + 8 * i + fc + e] = acc1[4 * i + 2 * hh + e];
                 }
-                br::tc_commit(&empty_bar[s]);
-                if (++s == NSTAGE) { s = 0; ph ^= 1; }
-            }
-            br::tc_commit(acc_bar);
-        }
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+#pragma unroll
+        for (int c = 0; c < NPAD; ++c) v[c] = s_t[row * (NPAD + 1) + c];
     } else {
-        const int lane_grp = warp & 3;
-        const int row = lane_grp * 32 + lane;
-        const int prow = tile * BM + row;                              // row of the product = feature index of `big`
-        const uint32_t taddr = tmem_base + ((uint32_t)(lane_grp * 32) << 16);
-        float v[NPAD];
-        if (n_kb > 0) {
-            br::mbar_wait(acc_bar, 0);
-            br::tc_fence_after();
 #pragma unroll
-            for (int c = 0; c < NPAD; c += 16) {
-                uint32_t r[16];
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                    : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                      "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                    : "r"(taddr + c) : "memory");
-                br::tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 16; ++i) v[c + i] = __uint_as_float(r[i]);
-            }
-        } else {
-#pragma unroll
-            for (int c = 0; c < NPAD; ++c) v[c] = 0.f;
-        }
+        for (int c = 0; c < NPAD; ++c) v[c] = 0.f;
+    }
+    {
         if (split != 0) {
             float* mine = p.ws + ((long long)blockIdx.x * NPAD) * BM + row;
 #pragma unroll
@@ -124,7 +123,7 @@ tn_gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             if (lane == 0) asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(p.counters + tile) : "memory");
         } else {
             if (p.splits > 1) {
-                if (threadIdx.x == 64) {
+                if (et == 0) {
                     const unsigned want = 4u * (unsigned)(p.splits - 1);
                     unsigned seen;
                     do { asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(p.counters + tile) : "memory"); } while (seen < want);
@@ -165,15 +164,13 @@ tn_gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             }
         }
     }
-    br::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) { br::tc_fence_after(); br::tmem_dealloc(tmem_base, NPAD <= 32 ? 32 : (NPAD <= 64 ? 64 : 128)); }
 }
 
 template <int NPAD>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, const TnParams& p, cudaStream_t st) {
-    constexpr int NBB = (NPAD + 63) / 64;
+    constexpr int NBB = NPAD / 64;
     constexpr int SMEM = NSTAGE * (A_BYTES + NBB * B_BLK) + 256 + 1024;
+    static_assert(NSTAGE * (A_BYTES + NBB * B_BLK) >= BM * (NPAD + 1) * 4, "transpose buffer");
     auto kern = tn_gemm_tc5_kernel<NPAD>;
     static bool done = false;
     if (!done) { BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM)); done = true; }
@@ -205,7 +202,7 @@ int br_lora_grad_tn(const void* big, int64_t ldb, const void* small, int64_t lds
         p.seg[i].col_lo = segs[i].col_lo; p.seg[i].n_cols = segs[i].n_cols;
         BR_CHECK_ARG(segs[i].dst && segs[i].col_lo >= 0 && segs[i].col_lo + segs[i].n_cols <= N, "lora_grad_tn: segment %d columns outside [0, N)", i);
     }
-    p.Npad = N <= 32 ? 32 : (N <= 64 ? 64 : (N <= 96 ? 96 : 128));
+    p.Npad = N <= 64 ? 64 : 128;                                  // MN-major wgmma operands come in 64-column swizzle atoms
     p.tiles = (P + BM - 1) / BM;
     p.kb_total = (M + BKT - 1) / BKT;
     int splits = br_num_sms() / p.tiles;                        // every CTA must be co-resident (the reducer spins on its peers)
@@ -222,12 +219,7 @@ int br_lora_grad_tn(const void* big, int64_t ldb, const void* small, int64_t lds
     if ((rc = br_make_tmap_2d_bf16(&ta, big, (uint64_t)M, (uint64_t)P, (uint64_t)ldb, BKT))) return rc;
     if ((rc = br_make_tmap_2d_bf16(&tb, small, (uint64_t)M, (uint64_t)N, (uint64_t)lds, BKT))) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    switch (p.Npad) {
-        case 32: return launch<32>(ta, tb, p, st);
-        case 64: return launch<64>(ta, tb, p, st);
-        case 96: return launch<96>(ta, tb, p, st);
-        default: return launch<128>(ta, tb, p, st);
-    }
+    return p.Npad == 64 ? launch<64>(ta, tb, p, st) : launch<128>(ta, tb, p, st);
 }
 
 }  // extern "C"

@@ -99,7 +99,7 @@ def _rope_table(n_pos: int, D: int, theta: float, device):
 
 
 def _lin(x, w, *, lora_a=None, lora_b=None, lora_scale=1.0, saved_t=None, **kw):
-    """y = x @ w.T (+ (scale * x @ A.T) @ B.T as a second K segment of the same tcgen05 accumulation)."""
+    """y = x @ w.T (+ (scale * x @ A.T) @ B.T as a second K segment of the same wgmma accumulation)."""
     if lora_a is None:
         return ops.gemm(x, w, **kw), None
     t = ops.gemm(x, lora_a, alpha=lora_scale)

@@ -246,11 +246,11 @@ class RolloutEngine:
             St.uniforms = uniforms.clone() if params.do_sample else None
             St.scratch = ops.skinny_scratch(max(cfg.vocab_size, 2 * cfg.intermediate_size), dev)
             # two KV tiles per work item where the co-residency cap allows it: both are fetched before the dependency wait, so the tile loop
-            # never waits on DRAM (measured: (14, 3) splits 2069 tok/s vs (8, 2) 2028 at 28 shared pages)
+            # never waits on DRAM
             ss_default = min(16, max(8, (n_shared + 1) // 2))
             splits_shared = min(int(os.environ.get("BR_ATTN_SS", ss_default)), n_shared) if n_shared > 0 else 0
             splits_private = int(os.environ.get("BR_ATTN_SP", 3)) if n_shared > 0 else 8
-            per_sm = 2 if os.environ.get("BR_DECODE_ATTN_TC5", "0") not in ("0", "") else 3     # CTAs of the fused attention an SM can hold
+            per_sm = 3                                                                  # CTAs of the fused attention an SM can hold (74 KB each)
             cap = per_sm * torch.cuda.get_device_properties(dev).multi_processor_count      # the fused kernel's merger items need co-residency
             n_items = lambda ss, sp: (R // G) * Hkv * ss + R * Hkv * sp
             while n_items(splits_shared, splits_private) > cap and (splits_shared > 1 or splits_private > 1):

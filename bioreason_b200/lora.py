@@ -149,7 +149,7 @@ class LoraState:
 @torch.no_grad()
 def build_rollout_weights(dec_w, lora: "LoraState | None", out=None):
     """Decode-time weights: W_eff = W + scale * B A per fused weight (the policy that rolls out is base + LoRA; merged with the
-    tcgen05 GEMM, base weight as the epilogue residual), with the RMSNorm gains folded into the columns of the matrices that
+    wgmma GEMM, base weight as the epilogue residual), with the RMSNorm gains folded into the columns of the matrices that
     consume a normed input (w_qkv <- ln1, w_gu <- ln2, lm_head <- final norm) so the decode step needs no norm launches."""
     from . import ops
     from .packing import DecoderLayerW, DecoderW

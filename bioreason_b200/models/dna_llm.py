@@ -1,4 +1,4 @@
-"""B200-native `DNALLMModel` -- same Python surface as bioreason/models/dna_llm.py:18-305, math in libbioreason_b200.
+"""CUDA-native `DNALLMModel` -- same Python surface as bioreason/models/dna_llm.py:18-305, math in libbioreason_b200.
 
 What is kept from the reference (SURVEY.md §8b): constructor kwargs, `forward(input_ids, attention_mask, dna_tokenized,
 batch_idx_map, labels=None, **kw)` returning an object with `.logits` / `.loss`, `generate(...)` returning completion-only
@@ -80,7 +80,7 @@ class DNALLMModel(nn.Module):
         if dna_is_evo2:
             raise NotImplementedError("Evo2 (StripedHyena-2) encoder is SURVEY.md §8f 'next'; NT-v2 is the path built here")
         if not torch.cuda.is_available():
-            raise RuntimeError("bioreason_b200.DNALLMModel needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("bioreason_b200.DNALLMModel needs a CUDA device (sm_90a); there is no CPU fallback")
         self.text_model_finetune, self.dna_model_finetune = text_model_finetune, dna_model_finetune
         self.max_length_dna, self.max_length_text = max_length_dna, max_length_text
         self.dna_is_evo2, self.dna_embedding_layer = dna_is_evo2, dna_embedding_layer

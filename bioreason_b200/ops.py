@@ -94,7 +94,7 @@ def _row_major_2d(t):
 def gemm(a: torch.Tensor, b: torch.Tensor, *, bias=None, residual=None, alpha: float = 1.0, act: int = 0,
          out: Optional[torch.Tensor] = None, out_dtype=torch.bfloat16, row_map=None, aux_out=None,
          a2=None, b2=None) -> torch.Tensor:
-    """out[M,N] = epilogue(a[M,K] @ b[N,K].T (+ a2[M,K2] @ b2[N,K2].T)) on tcgen05 (bf16 in, fp32 accumulate)."""
+    """out[M,N] = epilogue(a[M,K] @ b[N,K].T (+ a2[M,K2] @ b2[N,K2].T)) on wgmma (bf16 in, fp32 accumulate)."""
     _need_cuda(a, b)
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16
     M, K = a.shape
@@ -442,7 +442,7 @@ _LORA_WS = {}
 
 
 def lora_grad_tn(big, small, segs, *, mode=0):
-    """Deterministic tcgen05 TN GEMM: product[P, N] = big[M, P]^T @ small[M, N]; the blocks named by `segs` are ADDED into fp32 views.
+    """Deterministic wgmma TN GEMM: product[P, N] = big[M, P]^T @ small[M, N]; the blocks named by `segs` are ADDED into fp32 views.
     segs: list of (dst fp32 2-D view with contiguous rows, row_lo, row_hi, col_lo, n_cols); mode 1: one segment, dst[n, p] (transposed);
     mode 2: gate/up-blocked product rows (segment 0 = gate rows, 1 = up rows)."""
     _need_cuda(big, small)

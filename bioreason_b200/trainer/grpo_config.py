@@ -66,8 +66,8 @@ class DNALLMGRPOConfig:
     save_steps: int = 0                   # > 0: fire the callbacks' on_save every save_steps optimizer steps (HF save_strategy="steps")
     save_safetensors: bool = False        # reason.py:597 sets it; saving itself is the callbacks' job (reason.py:46-81)
     lora_dropout: float = 0.05            # accepted; the kernels apply no dropout (DESIGN.md: out of scope)
-    # B200 build additions
+    # additions of this implementation
     lora_r: int = 32
     lora_alpha: float = 64.0
-    micro_rows: Optional[int] = None      # rows per forward/backward chunk (None = all rows at once)
+    micro_rows: Optional[int] = None      # rows per forward/backward chunk (None = as many as the device memory holds)
     suppress_eos: bool = False            # fixed-length rollouts (bench config c)

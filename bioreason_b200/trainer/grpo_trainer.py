@@ -1,4 +1,4 @@
-"""B200-native `DNALLMGRPOTrainer`: the tensor math of bioreason/trainer/grpo_trainer.py on libbioreason_b200.
+"""CUDA-native `DNALLMGRPOTrainer`: the tensor math of bioreason/trainer/grpo_trainer.py on libbioreason_b200.
 
 Kept from the reference: `RepeatRandomSampler` semantics (:72-119), the rollout with the hard-coded sampling config
 (:384-391), EOS-inclusive completion mask (:605-609), ref log-probs with the frozen reference policy, old log-probs only
@@ -258,6 +258,17 @@ class DNALLMGRPOTrainer:
         return dict(prompt_ids=prompt_ids, prompt_mask=prompt_mask, completion_ids=completion_ids, completion_mask=completion_mask,
                     old_per_token_logps=old_lp, ref_per_token_logps=ref_lp, advantages=advantages, multimodal_inputs=mm)
 
+    @staticmethod
+    def _auto_micro_rows(model, B, L):
+        """Rows per forward/backward chunk when the config leaves `micro_rows` open: the most rows whose saved activations fit in
+        three quarters of the memory this process can still get -- free device memory (other processes' allocations excluded) plus
+        what the caching allocator holds but has not handed out; the rest is headroom for the backward's transients.  The loss is
+        row-separable, so the chunking changes only the fp32 order of the gradient sums."""
+        dev = model._dec.embed.device
+        free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+        per_row = L * training.activation_bytes_per_token(model)
+        return max(1, min(B, int(0.75 * free) // per_row))
+
     # ------------------------------------------------------------------ loss (+ backward through the kernels)
     def compute_loss(self, model, inputs, return_outputs=False, num_items_in_batch=None, backward: bool = True):
         if return_outputs:
@@ -276,7 +287,7 @@ class DNALLMGRPOTrainer:
         mask = torch.cat([prompt_mask, completion_mask.to(prompt_mask.dtype)], dim=1)
         B, C = completion_ids.shape
         adv, old, ref = inputs["advantages"], inputs["old_per_token_logps"], inputs["ref_per_token_logps"]
-        mr = self.args.micro_rows or B
+        mr = self.args.micro_rows or (self._auto_micro_rows(model, B, ids.shape[1]) if ids.is_cuda else B)
         ga = self.args.gradient_accumulation_steps
         loss_acc = torch.zeros(3, device=ids.device)
         for lo in range(0, B, mr):

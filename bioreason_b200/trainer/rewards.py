@@ -3,7 +3,7 @@
 The reference decodes the completions with `processing_class.batch_decode(..., skip_special_tokens=True)`, wraps them as
 `[{"role": "assistant", "content": text}]` when the examples are conversational, and calls every reward function as
 `reward_func(prompts=prompts, completions=completions, **columns)` where `columns` are the remaining keys of the examples
-(one list entry per row).  That protocol is the default here.  Two additions for the B200 path:
+(one list entry per row).  That protocol is the default here.  Two additions for the CUDA path:
 
 * a reward function may opt into the token-level fast path by NAMING a `completion_ids` parameter
   (`def f(completion_ids, completion_mask=None, prompt_ids=None, **kw)`): it then receives device tensors and nothing is

@@ -19,6 +19,19 @@ class PolicyCtx:
     pass
 
 
+def activation_bytes_per_token(model) -> int:
+    """Bytes `policy_forward(save=True)` keeps per token for the backward: per decoder layer the block input and its RMSNorm, the QKV
+    GEMM output, the roped q|k, the attention output and log-sum-exp, the mid-block residual and its RMSNorm, the gate|up
+    pre-activations and the SwiGLU output (bf16 unless noted), plus the LoRA intermediates."""
+    cfg = model._dec.cfg
+    d, F = cfg.hidden_size, cfg.intermediate_size
+    Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+    r = model._lora.r if getattr(model, "_lora", None) is not None else 0
+    bf16 = 2 * (4 * d + (Hq + 2 * Hkv) * D + (Hq + Hkv) * D + Hq * D + 2 * F + F + 4 * r)
+    fp32 = 4 * (2 + Hq)                                                    # two rstd values, one lse per query head
+    return cfg.num_hidden_layers * (bf16 + fp32) + 2 * d                   # + the final hidden state
+
+
 def policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_map, keep_last: int, *, save: bool = True,
                    lora="policy", targets: Optional[torch.Tensor] = None) -> "tuple[torch.Tensor, Optional[PolicyCtx]]":
     """Returns (logps [B, keep_last] fp32, ctx).  lora: "policy" (adapters on), None (base weights = reference policy).

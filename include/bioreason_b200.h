@@ -1,4 +1,4 @@
-/* libbioreason_b200 -- C ABI of the B200-native BioReason hot path.
+/* libbioreason_b200 -- C ABI of the sm_90a (H100) BioReason hot path.
  *
  * The reference (bowang-lab/BioReason) has no FFI: its hot path is Python calling HuggingFace/PyTorch
  * (SURVEY.md §8b).  This header is the boundary the build introduces *below* the reference's Python
@@ -29,7 +29,7 @@ extern "C" {
 int br_version(void);
 /* copies the calling thread's last error message into buf (NUL-terminated); returns its length */
 int br_last_error(char* buf, size_t n);
-/* 1 if the visible device is sm_100 (B200); the library refuses to run elsewhere */
+/* 1 if the visible device is sm_90 (H100); the library refuses to run elsewhere */
 int br_device_ok(void);
 
 /* ---------------------------------------------------------------------------------------------
@@ -47,7 +47,7 @@ int br_grpo_loss_fwd_bwd(const float* lp, const float* old_lp, const float* ref_
 int br_eos_mask(const int64_t* completion_ids, int B, int C, int64_t eos_id, int32_t* mask, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Dense contractions on tcgen05 (replaces every nn.Linear / lm_head reached through
+ * Dense contractions on wgmma (replaces every nn.Linear / lm_head reached through
  * dna_llm.py:150-160,237-242; SURVEY.md §2.3 K1,K2,K5,K6,K7,K12)
  * ------------------------------------------------------------------------------------------- */
 typedef struct br_gemm_epilogue {
@@ -137,7 +137,7 @@ int br_skinny_gemm_ex(const void* X, int64_t ldx, const void* W, int64_t ldw, vo
                       const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n, float* sumsq_out,
                       float eps, void* stream);
 /* L2 staging for the decode loop.  The decode step is a chain of small dependent kernels; while one of them waits on its predecessor or
- * reduces partial tiles, HBM idles.  A launch can therefore pull weight tiles of a LATER GEMM of the chain into the 126 MB L2:
+ * reduces partial tiles, HBM idles.  A launch can therefore pull weight tiles of a LATER GEMM of the chain into the 50 MB L2:
  * `W [N, K]` is that GEMM's weight, and of every chunk its CTAs will stream (the stream-K decomposition of br_skinny_gemm_ex) the 16 KB
  * tiles [unit_lo, unit_hi) are prefetched.  Weights are constant during a rollout, so this is safe at any point of the chain. */
 typedef struct br_l2_prefetch { const void* W; int64_t ldw; int32_t N, K; int32_t unit_lo, unit_hi; } br_l2_prefetch;
@@ -243,7 +243,7 @@ int br_swiglu_bwd(const void* gu, int64_t ldgu, const void* dact, int64_t ldda, 
 /* in place on the q and k head columns of dqkv: inverse RoPE then per-head RMSNorm backward (qk_pre = pre-norm q|k) */
 int br_qk_rope_bwd(void* dqkv, int64_t ldd, const void* qk_pre, int64_t ldp, int M, int n_q_heads, int n_k_heads, int head_dim,
                    const void* q_norm_w, const void* k_norm_w, const int32_t* positions, float theta, float eps, void* stream);
-/* LoRA weight gradients on tcgen05 (deterministic):  product[P, N] = big[M, P]^T . small[M, N] over the M tokens (both token-major,
+/* LoRA weight gradients on wgmma (deterministic):  product[P, N] = big[M, P]^T . small[M, N] over the M tokens (both token-major,
  * bf16, read as MN-major tensor-core operands), then  dst (+)= the blocks the segments name.
  *   mode 0: segment i adds product rows [row_lo, row_hi), columns [col_lo, col_lo + n_cols) into dst[(row - row_lo) * ld + col - col_lo]
  *           (dB of one adapter, or the q / k / v blocks of the fused qkv product);

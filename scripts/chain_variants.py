@@ -107,4 +107,4 @@ for mode in ("off", "on"):
             x2 = ops.skinny_gemm(attn_out, w["o"], scratch, mode=1, residual=x, sumsq_out=ssb, gate=g("o", False))
             a = ops.skinny_gemm(x2, w["gu"], scratch, mode=2, sumsq_in=ssb, sumsq_in_n=n_part, eps=1e-6, gate=g("gu", True))
             x = ops.skinny_gemm(a, w["down"], scratch, mode=1, residual=x2, sumsq_out=ssa, gate=g("down", True))
-    print(f"stream gate {mode:3s} (BR_SKINNY_PARK={os.environ.get('BR_SKINNY_PARK', '0')}): {timed(fn):7.2f} us per layer")
+    print(f"stream gate {mode:3s}: {timed(fn):7.2f} us per layer")

@@ -1,5 +1,5 @@
 """One representative launch of every hot kernel at config (c) shapes for `ncu --set full --profile-from-start off`:
-the big decoder GEMMs and the fused lm_head (tensor-bound), tcgen05 flash attention forward / backward, the LoRA-gradient TN GEMM,
+the big decoder GEMMs and the fused lm_head (tensor-bound), wgmma flash attention forward / backward, the LoRA-gradient TN GEMM,
 the decode weight-streaming GEMMs (HBM-bound) and the fused decode attention.  Everything is warmed up once outside the profiled range."""
 import math, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -35,7 +35,7 @@ def run():
     ops.gemm(act, w_down, residual=res)                  # down_proj + residual
     ops.lmhead_logprob(h_sel, emb, tgt)                  # fused lm_head + LSE (logits never in HBM)
     q, k, v = qkv[:, :Hq * D], qkv[:, Hq * D:(Hq + Hkv) * D], qkv[:, (Hq + Hkv) * D:]
-    o, lse = ops.attn_fwd(q, k, v, B, L, Hq, Hkv, D, causal=True, want_lse=True)                 # tcgen05 flash attention forward
+    o, lse = ops.attn_fwd(q, k, v, B, L, Hq, Hkv, D, causal=True, want_lse=True)                 # wgmma flash attention forward
     ops.attn_bwd(q, k, v, o, dout, lse, dqkv[:, :Hq * D], dqkv[:, Hq * D:(Hq + Hkv) * D], dqkv[:, (Hq + Hkv) * D:], B, L, Hq, Hkv, D)
     ops.lora_grad_tn(dqkv, t_qkv, [(g_q, 0, Hq * D, 0, r), (g_k, Hq * D, (Hq + Hkv) * D, r, r), (g_v, (Hq + Hkv) * D, NQ, 2 * r, r)])
     ops.lora_grad_tn(dgu, t_gu, [(g_gate, 0, 2 * F, 0, r), (g_up, 0, 2 * F, r, r)], mode=2)

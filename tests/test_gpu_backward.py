@@ -94,7 +94,7 @@ def test_attn_bwd(ops, B, L, nq, nkv):
 
 
 def test_lora_grad_tn_transpose_colsum(ops):
-    """The tcgen05 TN GEMM behind the LoRA gradients (both operands MN-major, split-K without atomics): all three epilogue modes,
+    """The wgmma TN GEMM behind the LoRA gradients (both operands MN-major, split-K without atomics): all three epilogue modes,
     accumulation into the destination, strided views, bit-reproducibility; plus the transpose and column-sum helpers."""
     torch.manual_seed(3)
     M, P = 1000, 512

@@ -127,33 +127,40 @@ def test_config_c_logps_grads_microrows_determinism():
         lp16 = torch.cat([_oracle_logps(o16, ids[r:r + 1], mask[r:r + 1], dict(dna_tokenized={k: v[2 * r:2 * r + 2] for k, v in mm["dna_tokenized"].items()},
                                                                                  batch_idx_map=[0, 0]), C).float() for r in range(G)])
     del o16
-    # ---- CUDA path
+    # ---- CUDA path, in row chunks: the activations one row keeps for the backward at L = 2364 are ~9 GB (Qwen3-4B, 36 layers), so the
+    #      8 rows do not fit next to the fp32 oracle on an 80 GB device.  Rows are independent in the forward and the loss is row-separable.
+    def chunked(rows_per_chunk):
+        lps = []
+        for lo in range(0, G, rows_per_chunk):
+            hi = lo + rows_per_chunk
+            idx = [i for i, b in enumerate(mm["batch_idx_map"]) if lo <= b < hi]
+            dna = {k: v[idx] for k, v in mm["dna_tokenized"].items()}
+            lp_c, ctx = training.policy_forward(m, ids[lo:hi], mask[lo:hi], dna, [mm["batch_idx_map"][i] - lo for i in idx], C)
+            training.policy_backward(m, ctx, wgt[lo:hi])
+            del ctx
+            lps.append(lp_c)
+        return torch.cat(lps)
+
     m.zero_grad_buffers()
-    lp, ctx = training.policy_forward(m, ids, mask, mm["dna_tokenized"], mm["batch_idx_map"], C)
+    lp = chunked(2)
     att = cmask.bool().cuda()
     e_mine, e_ref = (lp - lp_o)[att].abs(), (lp16 - lp_o)[att].abs()
     print(f"(c) logps L={ids.shape[1]}: max|err| ours {e_mine.max():.4f} vs HF-bf16 {e_ref.max():.4f}; mean {e_mine.mean():.5f} vs {e_ref.mean():.5f}")
     assert e_mine.mean().item() <= 1.25 * e_ref.mean().item() + 1e-4
     assert e_mine.max().item() <= 1.25 * e_ref.max().item() + 2e-2
-    training.policy_backward(m, ctx, wgt)
     worst, wname, rw, rb = _grad_report(m, oracle)
     print(f"(c) grads: worst LoRA rel err {worst:.4f} ({wname}); projector dW {rw:.4f} db {rb:.4f}")
     assert worst < 0.03 and rw < 0.03 and rb < 0.03
     # ---- bit-reproducibility of the whole backward (no floating-point atomics anywhere)
     g1 = lora.flat_grad.clone(); pw1 = m._proj_grad_w.clone()
     m.zero_grad_buffers()
-    lp_b, ctx = training.policy_forward(m, ids, mask, mm["dna_tokenized"], mm["batch_idx_map"], C)
-    training.policy_backward(m, ctx, wgt)
+    lp_b = chunked(2)
     assert torch.equal(lp_b, lp)
     assert torch.equal(lora.flat_grad, g1) and torch.equal(m._proj_grad_w, pw1), "gradients are not run-to-run reproducible"
-    # ---- micro_rows chunking == unchunked (row-separable loss; only the fp32 accumulation order across chunks differs)
+    # ---- micro_rows chunking: one-row chunks == two-row chunks (row-separable loss; only the fp32 accumulation order differs)
     m.zero_grad_buffers()
-    for lo in range(0, G, 4):
-        idx = [i for i, b in enumerate(mm["batch_idx_map"]) if lo <= b < lo + 4]
-        dna = {k: v[idx] for k, v in mm["dna_tokenized"].items()}
-        lp_c, ctx = training.policy_forward(m, ids[lo:lo + 4], mask[lo:lo + 4], dna, [mm["batch_idx_map"][i] - lo for i in idx], C)
-        assert (lp_c - lp[lo:lo + 4]).abs().max().item() < 1e-4           # forward rows are independent of the chunking
-        training.policy_backward(m, ctx, wgt[lo:lo + 4])
+    lp_c = chunked(1)
+    assert (lp_c - lp).abs().max().item() < 1e-4                           # forward rows are independent of the chunking
     assert _rel(lora.flat_grad, g1) < 2e-3 and _rel(m._proj_grad_w, pw1) < 2e-3
 
 

@@ -1,4 +1,4 @@
-"""GPU parity tests for the C-ABI kernels (run with -m gpu on a B200)."""
+"""GPU parity tests for the C-ABI kernels (run with -m gpu on an H100)."""
 import os, ctypes
 import numpy as np
 import pytest
