@@ -54,7 +54,7 @@ def last_error() -> str:
     return ffi.string(buf).decode()
 
 
-_KERNELS_PER_CALL = {"lmhead_logprob_fwd": 2, "attn_bwd": 2, "decode_attn": 3, "sample_next_2stage": 2, "skinny_chain": 1}
+_KERNELS_PER_CALL = {"lmhead_logprob_fwd": 2, "attn_bwd": 2, "sample_next_2stage": 2}
 COUNTER = [0]
 
 

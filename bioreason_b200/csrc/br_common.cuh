@@ -92,7 +92,7 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, ui
         : "memory");
 }
 
-// same with an L2 eviction-priority hint (policy from make_policy_evict_first / _last)
+// same with an L2 eviction-priority hint (policy from make_policy_evict_first)
 __device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, uint64_t policy) {
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(
@@ -102,29 +102,6 @@ __device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const void* tma
 }
 __device__ __forceinline__ uint64_t make_policy_evict_first() {
     uint64_t p; asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p)); return p;
-}
-__device__ __forceinline__ uint64_t make_policy_evict_last() {
-    uint64_t p; asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p)); return p;
-}
-
-// pull one box of a tiled tensor into L2 only (no shared-memory destination, no barrier)
-__device__ __forceinline__ void tma_prefetch_l2_2d(const void* tmap, int c0, int c1) {
-    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(tmap), "r"(c0), "r"(c1) : "memory");
-}
-// L2 staging of a LATER decode GEMM's weights: for every chunk c of that GEMM's stream-K decomposition (chunk = units one of its CTAs
-// streams, unit = one 128-feature x 64-k tile of 16 KB in streaming order) pull units [a, b) of the chunk into L2.  Called by ONE
-// thread of each CTA of an EARLIER kernel whose own demand for HBM is low; the consumer then streams those tiles at L2 speed.
-struct L2Prefetch { int KB, units, chunk, n_chunks, a, b; };
-__device__ __forceinline__ void l2_prefetch_issue(const void* tmap, const L2Prefetch& pf, int cta, int n_cta) {
-    for (int c = cta; c < pf.n_chunks; c += n_cta) {
-        const int u_end = min(pf.units, (c + 1) * pf.chunk);
-        for (int j = pf.a; j < pf.b; ++j) {
-            const int u = c * pf.chunk + j;
-            if (u >= u_end) break;
-            const int tile = u / pf.KB, kb = u - tile * pf.KB;
-            tma_prefetch_l2_2d(tmap, kb * 64, tile * 128);
-        }
-    }
 }
 
 // generic-proxy shared-memory writes -> visible to the async proxy (wgmma / TMA reading shared memory)
@@ -174,10 +151,6 @@ static inline cudaError_t br_launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 
     return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 #endif
-
-// Host: decomposition of a decode GEMM [N, K] exactly as br_skinny_gemm_ex cuts it (decode_gemm_tc5.cu), for l2_prefetch_issue
-struct br_l2_prefetch;
-int br_make_l2_prefetch(const struct br_l2_prefetch* spec, CUtensorMap* tmap, int* KB, int* units, int* chunk, int* n_chunks, int* a, int* b);
 
 // Host: 2-D bf16 row-major tensor map, box = {64 cols (128 B, SWIZZLE_128B), box_rows}
 int br_make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows);

@@ -1,6 +1,15 @@
-// One launch per layer per decode step: q/k RMSNorm + RoPE, KV append, prefix-shared + private paged attention and the
-// split combine (replaces br_decode_rope_append + the two br_decode_attn passes + the combine kernel: 4 launches -> 1;
-// the decode step is launch-latency sensitive -- ~360 small launches per token before fusion).
+// Paged-KV decode attention for the GRPO rollout (replaces the HF generate() token loop + DynamicCache torch.cat growth,
+// HF generation/utils.py:2760-2800; SURVEY.md §2.3 K8).
+//
+// KV cache layout (per layer): K and V are [n_pages, Hkv, 64, D] bf16 -- the 64 keys of one (page, kv head) are one
+// contiguous 16 KB tile, i.e. exactly the shared-memory tile of the attention kernel.  A row's context is a page
+// table; the G samples of a prompt group point at the SAME prompt pages (prefix sharing), so the shared-prefix pass treats
+// the whole group as one problem (G x Hq/Hkv query vectors per kv head form the M dimension of the QK^T / PV mma tiles) and
+// reads every prompt K/V tile once per group instead of G times.  Everything that changes from step to step (row lengths) is
+// read from device memory, so one captured CUDA graph replays for every token.
+//
+// One launch per layer per decode step (the decode step is launch-latency sensitive): q/k RMSNorm + RoPE, KV append,
+// prefix-shared + private paged attention and the split combine.
 //
 // Work items (blockIdx.x): first  n_groups*Hkv*SS  "shared" items  (group, kv head, split over the common prompt pages;
 //                                 G x Hq/Hkv query vectors = the M dimension of the mma tiles),
@@ -14,9 +23,6 @@
 using namespace attn;
 
 namespace {
-
-__device__ __forceinline__ long long gtime() { long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-#define STAMP(k) do { if (p.dbg && tid == 0) p.dbg[(long long)blockIdx.x * 16 + (k)] = gtime(); } while (0)
 
 __device__ __forceinline__ float rbf(float x) { return __bfloat162float(__float2bfloat16(x)); }
 // two roundings with ONE conversion instruction (F2FP packs a pair; it issues at the special-function rate, so a prologue made of
@@ -34,10 +40,8 @@ struct FusedParams {
     float* part_o; float* part_lse; int* counters;      // [R,Hq,n_slots,D], [R,Hq,n_slots], [2][R*Hkv] (arrivals, finished pollers)
     bf16* out; long long ldo;
     float scale_log2, theta, eps;
-    long long* dbg;                      // optional [items, 16] globaltimer stamps (profiling aid)
     const float2* rope;                  // [n_pos, D/2] (cos, sin), bf16-rounded like HF's tables
     int rope_n_pos;
-    br::L2Prefetch pf; int pf_on;        // L2 staging of a later GEMM's weights (see br_common.cuh)
 };
 
 // cos/sin table: rope[pos, j] = (bf16(cos(pos * theta^(-2j/D))), bf16(sin(...))) -- the transcendental work of the decode loop, done once
@@ -49,6 +53,22 @@ __global__ void rope_table_kernel(float2* __restrict__ out, int n_pos, int half,
     float sn, cs;
     sincosf((float)pos * inv_freq, &sn, &cs);
     out[i] = make_float2(rbf(cs), rbf(sn));
+}
+
+// prefill: copy the (already roped) K and V of tokens [0, n_tok) of one prompt row into its pages
+template <int D>
+__global__ void kv_write_pages_kernel(const bf16* __restrict__ qkv, long long ld, int n_tok, int Hq, int Hkv, const int* __restrict__ pages,
+                                      bf16* __restrict__ kcache, bf16* __restrict__ vcache) {
+    const int wid = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (wid >= n_tok * 2 * Hkv) return;
+    const int tok = wid / (2 * Hkv), hh = wid % (2 * Hkv);
+    const bool is_v = hh >= Hkv;
+    const int kvh = is_v ? hh - Hkv : hh;
+    const bf16* src = qkv + (long long)tok * ld + (long long)(Hq + hh) * D;
+    const int page = pages[tok >> 6], slot = tok & 63;
+    bf16* dst = (is_v ? vcache : kcache) + (((long long)page * Hkv + kvh) * 64 + slot) * D;
+    for (int i = lane; i < D / 8; i += 32) reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(src)[i];
 }
 
 // same arithmetic with the norm weights and the (cos, sin) pairs already in registers
@@ -109,7 +129,7 @@ __device__ __forceinline__ void load_head_words(const bf16* src, int lane, uint3
 // The two contractions of a tile run on mma.sync m16n8k16: the M dimension here is at most 32 query vectors, below the 64 rows of
 // a Hopper warpgroup MMA.
 template <int D>
-__global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, const __grid_constant__ CUtensorMap tmP) {
+__global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p) {
     constexpr int BN = 64, TILE = 64 * D * 2, NT = 64, QROWS = 32, E = D / 64;
     extern __shared__ __align__(128) uint8_t smem_raw[];
     uint8_t* smem = smem_raw;
@@ -119,7 +139,6 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
     auto qptr = [&](int s, int c) -> uint8_t* { return tile_ptr<D>(sQ, s, c); };
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
-    STAMP(0);
     br::launch_dependents();
     // ------------------------------------------------------------------------------------------------------------------
     // Everything up to grid_dep_wait() depends only on state the PREVIOUS kernel of the chain (this step's qkv GEMM) does not
@@ -161,8 +180,6 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
     if (early0) issue_tile(0, pg_lo);
     if (early1) issue_tile(1, pg1);
     cp_async_commit();
-    // this kernel moves ~17 MB per layer and spends most of its life waiting: its CTAs stage weight tiles of a later GEMM into L2
-    if (p.pf_on && tid == 0) br::l2_prefetch_issue(&tmP, p.pf, blockIdx.x, gridDim.x);
 
     // query-prep operands that do not depend on the new tokens: positions, norm weights, the rope pairs of the first pass.
     // NOTE on code size: this prologue runs once per CTA, so every instruction is a cold instruction-cache fetch; the 4 passes are a
@@ -199,7 +216,6 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
         }
     }
     br::grid_dep_wait();
-    STAMP(1);
 
     // ---- everything that depends on this step's qkv GEMM is requested at once: the raw query chunks and the new token's K / V
     {
@@ -220,7 +236,6 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
             if (warp == 0) load_head_words(p.qkv + (long long)row_base * p.ld + (long long)(p.Hq + kvh) * D, lane, kwlo, kwhi);
             else if (lane < D / 8) vraw = __ldcg(reinterpret_cast<const uint4*>(p.qkv + (long long)row_base * p.ld + (long long)(p.Hq + p.Hkv + kvh) * D) + lane);
         }
-        STAMP(8);
         // ---- queries: norm + rope (slot s -> row s / GQ, head kvh*GQ + s % GQ); 8 lanes per vector, 4 vectors per warp per pass, straight
         // from the registers the raw chunks landed in to their final (swizzled) place in the Q tile.  Slots are ordered by row: the passes
         // that hold a live query vector form a prefix (private items: ONE pass of warp 0, none of warp 1); dead slots get zeros.
@@ -252,7 +267,6 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
             *reinterpret_cast<uint4*>(qptr(s, sub)) = olo;
             *reinterpret_cast<uint4*>(qptr(s, 8 + sub)) = ohi;
         }
-        STAMP(9);
         // ---- append the new token's K / V (private item that owns the newest page)
         if (owns_newest) {
             const int pos = kv_len - 1;
@@ -272,7 +286,6 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
         }
     }
     __syncthreads();
-    STAMP(2);
     // the newest page, if it is one of the first two tiles of this item, could not be fetched before the append
     if (have0 && !early0) issue_tile(0, pg_lo);
     if (have1 && !early1) issue_tile(1, pg1);
@@ -286,7 +299,6 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
         ldsm_x4(qf[kk], tile_ptr<D>(sQ, warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, kk * 2 + (lane >> 4)));
     cp_async_wait<0>();
     __syncthreads();
-    STAMP(3);
 
     float o[D / 8][4];
 #pragma unroll
@@ -362,7 +374,6 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
         __syncthreads();
     }
 
-    STAMP(4);
     // ---- partials
     if (warp_live) {
         l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
@@ -386,7 +397,6 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
         }
     }
     }
-    STAMP(5);
     // ---- arrival counters: one per (row, kv head).  Every item publishes its partial and arrives; the SP private items of a
     //      (row, kv head) pair then ALL merge -- each a contiguous share of the pair's GQ x D output -- so the 64 merges of a step run on
     //      64 x SP CTAs and every thread has its whole gather (<= 32 slots of one float4 column) in flight in one L2 round trip.
@@ -401,7 +411,7 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
         if (lane < (shared_pass ? rows_in_warp : 1) && rr < rows_per_unit && row_base + rr < p.R)
             asm volatile("red.release.gpu.global.add.s32 [%0], 1;" ::"l"(p.counters + (row_base + rr) * p.Hkv + kvh) : "memory");
     }
-    if (shared_pass) { STAMP(6); STAMP(7); return; }
+    if (shared_pass) return;
     if (tid == 0) {
         int* c = p.counters + row_base * p.Hkv + kvh;
         int seen;
@@ -411,7 +421,6 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
         if (atomicAdd(dn, 1) == p.SP - 1) { *c = 0; *dn = 0; }
     }
     __syncthreads();
-    STAMP(6);
     {
         // Every thread owns one float4 column of one head: it loads the head's slot LSEs itself (the same addresses across the threads
         // of a head: broadcast) together with its column of every slot -- ONE L2 round trip -- and derives the slot weights redundantly
@@ -453,17 +462,21 @@ __global__ void __launch_bounds__(64) decode_fused_kernel(const FusedParams p, c
                 make_uint2(br::pack_bf16(acc.x, acc.y), br::pack_bf16(acc.z, acc.w));
         }
     }
-    STAMP(7);
 }
 
 }  // namespace
 
-static long long* g_dbg = nullptr;
-
 extern "C" {
 
-/* profiling aid: [items, 8] int64 globaltimer stamps written by the next br_decode_attn_fused launches (NULL disables) */
-int br_decode_attn_fused_debug(long long* buf) { g_dbg = buf; return BR_OK; }
+int br_kv_write_pages(const void* qkv, int64_t ld, int n_tok, int n_q_heads, int n_kv_heads, int head_dim, const int32_t* pages, void* kcache,
+                      void* vcache, void* stream) {
+    BR_CHECK_ARG(head_dim == 128 && n_tok > 0, "kv_write_pages: head_dim 128, n_tok > 0");
+    const int warps = n_tok * 2 * n_kv_heads, wpb = 8;
+    kv_write_pages_kernel<128><<<(warps + wpb - 1) / wpb, wpb * 32, 0, (cudaStream_t)stream>>>((const bf16*)qkv, ld, n_tok, n_q_heads, n_kv_heads,
+                                                                                             pages, (bf16*)kcache, (bf16*)vcache);
+    BR_CHECK_LAUNCH();
+    return BR_OK;
+}
 
 int64_t br_decode_fused_workspace_bytes(int R, int n_q_heads, int n_kv_heads, int head_dim, int n_slots) {
     return (int64_t)R * n_q_heads * n_slots * (head_dim + 1) * sizeof(float) + 2 * (int64_t)R * n_kv_heads * sizeof(int);
@@ -481,16 +494,6 @@ int br_decode_attn_fused(const void* qkv_raw, int64_t ld, const void* q_norm_w, 
                          const int32_t* page_table, int max_pages, const int32_t* cur_len, int R, int G, int n_q_heads, int n_kv_heads,
                          int head_dim, int n_shared_pages, int splits_shared, int splits_private, float scale, float theta, float eps,
                          const float* rope_table, int rope_n_pos, void* workspace, void* out, int64_t ldo, void* stream) {
-    return br_decode_attn_fused_pf(qkv_raw, ld, q_norm_w, k_norm_w, kcache, vcache, page_table, max_pages, cur_len, R, G, n_q_heads, n_kv_heads,
-                                   head_dim, n_shared_pages, splits_shared, splits_private, scale, theta, eps, rope_table, rope_n_pos, workspace,
-                                   out, ldo, nullptr, stream);
-}
-
-int br_decode_attn_fused_pf(const void* qkv_raw, int64_t ld, const void* q_norm_w, const void* k_norm_w, void* kcache, void* vcache,
-                            const int32_t* page_table, int max_pages, const int32_t* cur_len, int R, int G, int n_q_heads, int n_kv_heads,
-                            int head_dim, int n_shared_pages, int splits_shared, int splits_private, float scale, float theta, float eps,
-                            const float* rope_table, int rope_n_pos, void* workspace, void* out, int64_t ldo, const br_l2_prefetch* prefetch,
-                            void* stream) {
     BR_CHECK_ARG(head_dim == 128, "decode_attn_fused: head_dim 128 only");
     BR_CHECK_ARG(R > 0 && G > 0 && R % G == 0 && G <= 64, "decode_attn_fused: R=%d must be a multiple of G=%d (<= 64)", R, G);
     const int GQ = n_q_heads / n_kv_heads;
@@ -510,7 +513,6 @@ int br_decode_attn_fused_pf(const void* qkv_raw, int64_t ld, const void* q_norm_
     p.counters = (int*)(p.part_lse + (int64_t)R * n_q_heads * p.n_slots);
     p.out = (bf16*)out; p.ldo = ldo; p.scale_log2 = scale * 1.4426950408889634f; p.theta = theta; p.eps = eps;
     p.rope = (const float2*)rope_table; p.rope_n_pos = rope_table ? rope_n_pos : 0;
-    p.dbg = g_dbg;
     constexpr int SMEM = 32 * D * 2 + 4 * 64 * D * 2;
     static bool done = false;
     if (!done) {
@@ -520,15 +522,7 @@ int br_decode_attn_fused_pf(const void* qkv_raw, int64_t ld, const void* q_norm_
     const int items = (use_shared ? (R / G) * n_kv_heads * p.SS : 0) + R * n_kv_heads * p.SP;
     const int per_sm = 3;
     BR_CHECK_ARG(items <= per_sm * br_num_sms(), "decode_attn_fused: %d work items exceed the co-resident capacity (%d per SM) the in-kernel merge relies on", items, per_sm);
-    CUtensorMap tp;
-    memset(&tp, 0, sizeof(tp));
-    p.pf_on = 0;
-    if (prefetch && prefetch->W && prefetch->unit_hi > prefetch->unit_lo) {
-        int rc = br_make_l2_prefetch(prefetch, &tp, &p.pf.KB, &p.pf.units, &p.pf.chunk, &p.pf.n_chunks, &p.pf.a, &p.pf.b);
-        if (rc) return rc;
-        p.pf_on = 1;
-    }
-    BR_CHECK_CUDA(br_launch_pdl(decode_fused_kernel<D>, dim3(items), dim3(64), (size_t)SMEM, (cudaStream_t)stream, p, tp));
+    BR_CHECK_CUDA(br_launch_pdl(decode_fused_kernel<D>, dim3(items), dim3(64), (size_t)SMEM, (cudaStream_t)stream, p));
     return BR_OK;
 }
 

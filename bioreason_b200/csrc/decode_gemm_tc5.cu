@@ -31,17 +31,12 @@ struct SkParams {
     int mode;                           // 0 bf16, 1 bf16 + residual, 2 SwiGLU blocks, 3 fp32
     void* out; long long ldo;
     const bf16* res; long long ldr;
-    float* scratch;                     // [grid, 2, BNX, 128] fp32 partial tiles (slot 0: CTA's first tile, 1: its last tile)
+    float* scratch;                     // [grid, 32, 128] fp32: the partial tile each contributing CTA publishes (its chunk's first segment)
     int* counters;                      // [tiles_n], zero between launches (self-resetting)
     // folded RMSNorm (decode): out[r, :] *= rsqrt(sum_i sumsq_in[i, r] / K + eps) (the norm weight is pre-multiplied into W's
     // columns); sumsq_out[(tile*4 + warp), r] = sum over that warp's 32 features of out[r, f]^2 (bf16-rounded) -- partials are
     // written, never accumulated with atomics, and summed in a fixed order by the consumer: the rollout is reproducible.
     const float* sumsq_in; int sumsq_in_n; float* sumsq_out; float eps;
-    long long* dbg; int dbg_slot;       // optional %globaltimer stamps [slot][cta][8] (profiling aid)
-    br::L2Prefetch pf; int pf_on;       // L2 staging of a later GEMM's weights (see br_common.cuh)
-    int* gate_counter; const int* gate_epoch; int gate_base, gate_per_step, gate_wait, gate_signal;   // stream gate (see br_stream_gate)
-    int w_evict_first;                  // weight tiles are read once per token step: mark them evict-first in L2 so the small
-                                        // latency-critical buffers (activations, partial tiles, statistics, tables) stay resident
 };
 
 __device__ __forceinline__ float rbf(float x) { return __bfloat162float(__float2bfloat16(x)); }
@@ -63,7 +58,7 @@ struct SL {
 // the tile for every row (the layout the epilogue and the stream-K exchange work in).  Called by the consumer warpgroup (warps 0..3).
 template <int BNX, int RM>
 __device__ __forceinline__ void mma_tile(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, int& s, uint32_t& ph, int n_units,
-                                         int* signal_counter, float* s_tr, float (&v)[RM]) {
+                                         float* s_tr, float (&v)[RM]) {
     using L = SL<BNX>;
     const int et = threadIdx.x, warp = et >> 5, lane = et & 31;
     float acc0[BNX / 2], acc1[BNX / 2];
@@ -71,8 +66,6 @@ __device__ __forceinline__ void mma_tile(uint8_t* smem, uint64_t* full_bar, uint
     for (int i = 0; i < BNX / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
     for (int i = 0; i < n_units; ++i) {
         br::mbar_wait(&full_bar[s], ph);
-        if (i == n_units - 1 && signal_counter && et == 0)                    // every weight tile of this CTA is on chip
-            asm volatile("red.relaxed.gpu.global.add.s32 [%0], 1;" ::"l"(signal_counter) : "memory");
         const uint32_t sa = br::smem_u32(smem + s * L::STAGE);
         const uint64_t bdesc = br::wg_desc_k(sa + L::A_BYTES);
         br::wg_fence();
@@ -189,32 +182,27 @@ __device__ __forceinline__ void compute_row_rstd(const SkParams& p, int et, floa
     asm volatile("bar.sync 1, 128;" ::: "memory");
 }
 
-__device__ __forceinline__ long long gtime_sk() { long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-#define SKSTAMP(k) do { if (p.dbg && (threadIdx.x == 0)) p.dbg[((long long)p.dbg_slot * 160 + blockIdx.x) * 8 + (k)] = gtime_sk(); } while (0)
-
 
 // BNX: wgmma N (rows of X the tensor core sees, zero-filled beyond R); RM: rows the epilogue code is generated for (R <= RM <= BNX).
 // The epilogue runs once per CTA per launch -- straight-line, instruction-fetch-bound code -- so the common R <= 8 decode batch gets its
 // own half-size instantiation.  Warps 0..3: wgmma + epilogue (one feature row per thread), warp 4: TMA producer.
 template <int BNX, int RM>
 __global__ void __launch_bounds__(NTHREADS, 1)
-skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmP,
-                  const SkParams p) {
+skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX,
+                  const __grid_constant__ SkParams p) {      // read in place by the helpers (const SkParams&): no register copy
     using L = SL<BNX>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     float* s_tr = reinterpret_cast<float*>(smem + L::TILE_BYTES);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::TILE_BYTES + L::TR_BYTES);
     uint64_t* empty_bar = full_bar + L::NSTAGE;
-    int* s_flag = reinterpret_cast<int*>(empty_bar + L::NSTAGE);
-    float* s_rs = reinterpret_cast<float*>(s_flag + 2);       // [32] per-row rstd of the folded RMSNorm (+ [4][32] scratch)
+    float* s_rs = reinterpret_cast<float*>(empty_bar + L::NSTAGE);   // [32] per-row rstd of the folded RMSNorm (+ [4][32] scratch)
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int u_lo = blockIdx.x * p.chunk;
     const int u_hi = min(p.units, u_lo + p.chunk);
 
     br::launch_dependents();
-    SKSTAMP(0);
     if (threadIdx.x == 0) {
         br::tma_prefetch_desc(&tmW);
         br::tma_prefetch_desc(&tmX);
@@ -229,25 +217,14 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
             // The weights are constant during the rollout: fill the whole ring with weight tiles BEFORE waiting for the
             // previous kernel (PDL), so the HBM stream of this layer overlaps the tail of the previous kernel.
             const int n_pre = min(L::NSTAGE, n_units);
+            // weight tiles are read once per token step: evict-first in L2, so the small latency-critical buffers (activations,
+            // partial tiles, statistics, tables) stay resident
             const uint64_t pol = br::make_policy_evict_first();
-            if (p.gate_counter && p.gate_wait >= 0) {             // start the early loads under the previous GEMM's exchange tail, not under its stream
-                const int target = (__ldcg(p.gate_epoch) - p.gate_base) * p.gate_per_step + p.gate_wait;
-                for (int it = 0; it < 32; ++it) {                 // bounded: the gate is a timing hint
-                    int seen;
-                    asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(seen) : "l"(p.gate_counter) : "memory");
-                    if (seen >= target) break;
-                }
-            }
-            auto load_w = [&](void* dst, uint64_t* bar, int c0, int c1) {
-                if (p.w_evict_first) br::tma_load_2d_hint(dst, &tmW, bar, c0, c1, pol);
-                else br::tma_load_2d(dst, &tmW, bar, c0, c1);
-            };
             for (int i = 0; i < n_pre; ++i) {
                 const int u = u_lo + i, tile = u / p.KB, kb = u - tile * p.KB;
                 br::mbar_expect_tx(&full_bar[i], L::STAGE);
-                load_w(smem + i * L::STAGE, &full_bar[i], kb * BK, tile * BM);
+                br::tma_load_2d_hint(smem + i * L::STAGE, &tmW, &full_bar[i], kb * BK, tile * BM, pol);
             }
-            if (p.pf_on) br::l2_prefetch_issue(&tmP, p.pf, blockIdx.x, gridDim.x);     // a LATER GEMM's tiles -> L2 (HBM is otherwise idle here)
             br::grid_dep_wait();
             for (int i = 0; i < n_pre; ++i) {
                 const int u = u_lo + i, tile = u / p.KB, kb = u - tile * p.KB;
@@ -259,7 +236,7 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                 br::mbar_wait(&empty_bar[s], ph ^ 1);
                 uint8_t* sa = smem + s * L::STAGE;
                 br::mbar_expect_tx(&full_bar[s], L::STAGE);
-                load_w(sa, &full_bar[s], kb * BK, tile * BM);
+                br::tma_load_2d_hint(sa, &tmW, &full_bar[s], kb * BK, tile * BM, pol);
                 br::tma_load_2d(sa + L::A_BYTES, &tmX, &full_bar[s], kb * BK, 0);
                 if (++s == L::NSTAGE) { s = 0; ph ^= 1; }
             }
@@ -267,9 +244,7 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
     } else {
         const int lane_grp = warp & 3;
         const int et = threadIdx.x;                               // 0..127 within the consumer warpgroup
-        SKSTAMP(2);                                               // barriers initialised
         br::grid_dep_wait();                                      // everything below touches data shared with earlier kernels
-        SKSTAMP(1);
         compute_row_rstd(p, et, s_rs, s_rs + 32);
         int s = 0; uint32_t ph = 0;
         int u = u_lo;
@@ -282,9 +257,7 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
             float res[RM];
             load_residual<RM>(p, f, res);                        // in flight while the accumulator is still being produced
             float v[RM];
-            mma_tile<BNX, RM>(smem, full_bar, empty_bar, s, ph, seg_end - u, (seg_end == u_hi && p.gate_counter && p.gate_signal) ? p.gate_counter : nullptr,
-                              s_tr, v);
-            if (u == u_lo) SKSTAMP(3);
+            mma_tile<BNX, RM>(smem, full_bar, empty_bar, s, ph, seg_end - u, s_tr, v);
             if (whole) {
                 apply_epilogue<RM>(p, f, lane, v, res, s_rs, part_row);
             } else {
@@ -296,13 +269,12 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                 // to its own registers in ascending CTA order -- no floating-point atomics, bit-reproducible.
                 const int first_c = (tile * p.KB) / p.chunk, last_c = ((tile + 1) * p.KB - 1) / p.chunk;
                 if ((int)blockIdx.x != first_c) {
-                    float* mine = p.scratch + ((long long)blockIdx.x * 2 * BNX) * BM + lane_grp * 32 + lane;   // slot 0: the CTA's first tile
+                    float* mine = p.scratch + (long long)blockIdx.x * 32 * BM + lane_grp * 32 + lane;
     #pragma unroll
                     for (int r = 0; r < RM; ++r)
                         if (r < p.R) __stcg(mine + r * BM, v[r]);
                     __syncwarp();
                     if (lane == 0) asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(p.counters + tile) : "memory");
-                    if (seg_end == u_hi) SKSTAMP(4);
                 } else {
                     if (et == 0) {
                         const unsigned want = 4u * (unsigned)(last_c - first_c);
@@ -311,7 +283,6 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                         p.counters[tile] = 0;                                    // nobody touches it again before the next launch
                     }
                     asm volatile("bar.sync 1, 128;" ::: "memory");
-                    SKSTAMP(4);
                     for (int c0 = first_c + 1; c0 <= last_c; c0 += 8) {          // 8 contributors x 8 rows of loads in flight
     #pragma unroll
                         for (int r0 = 0; r0 < RM; r0 += 8) {
@@ -319,7 +290,7 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                             float t[8][8];
     #pragma unroll
                             for (int j = 0; j < 8; ++j) {
-                                const float* src = p.scratch + ((long long)(c0 + j) * 2 * BNX) * BM + lane_grp * 32 + lane;
+                                const float* src = p.scratch + (long long)(c0 + j) * 32 * BM + lane_grp * 32 + lane;
     #pragma unroll
                                 for (int r = 0; r < 8; ++r) t[j][r] = (c0 + j <= last_c && r0 + r < p.R) ? __ldcg(src + (r0 + r) * BM) : 0.f;
                             }
@@ -329,19 +300,16 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                                 for (int r = 0; r < 8; ++r) v[r0 + r] += t[j][r];            // ascending CTA order: deterministic
                         }
                     }
-                    SKSTAMP(5);
                     apply_epilogue<RM>(p, f, lane, v, res, s_rs, part_row);
-                    SKSTAMP(6);
                 }
             }
             u = seg_end;
         }
-        SKSTAMP(7);
     }
 }
 
 template <int BNX, int RM>
-int launch(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& tp, const SkParams& p, int grid, cudaStream_t st) {
+int launch(const CUtensorMap& tw, const CUtensorMap& tx, const SkParams& p, int grid, cudaStream_t st) {
     using L = SL<BNX>;
     auto kern = skinny_tc5_kernel<BNX, RM>;
     static bool done = false;
@@ -349,250 +317,31 @@ int launch(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& tp, 
         BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
         done = true;
     }
-    BR_CHECK_CUDA(br_launch_pdl(kern, dim3(grid), dim3(NTHREADS), (size_t)L::TOTAL, st, tw, tx, tp, p));
-    return BR_OK;
-}
-
-
-// ================================================================================================================
-// Multi-phase persistent variant: up to 4 dependent GEMMs (o_proj -> gate/up -> down_proj -> next layer's qkv, or
-// ... -> lm_head) in ONE launch.  Phases are separated by a grid-wide barrier instead of a kernel boundary; the weight
-// producer is not gated by the barrier, so while the CTAs synchronise (and while the last tiles of a phase are reduced)
-// the ring already fills with the next phase's weights -- the HBM stream does not stop at phase boundaries.  A second
-// producer thread loads the activation tiles and is the only one that waits for "phase inputs ready".
-// ================================================================================================================
-constexpr int CHAIN_MAX = 4;
-constexpr int CHAIN_THREADS = 192;           // warps 0-3: wgmma + epilogue, 4: W producer, 5: X producer
-
-struct ChainPhase { CUtensorMap tmW; CUtensorMap tmX; SkParams p; };
-struct ChainParams { ChainPhase ph[CHAIN_MAX]; int n_phases; int* gbar; long long* dbg; };
-__device__ __forceinline__ long long gtime() { long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-#define CSTAMP(k) do { if (cp.dbg && et == 0) cp.dbg[(long long)blockIdx.x * 32 + (k)] = gtime(); } while (0)
-
-template <int BNX>
-__global__ void __launch_bounds__(CHAIN_THREADS, 1) skinny_chain_kernel(const __grid_constant__ ChainParams cp) {
-    using L = SL<BNX>;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    float* s_tr = reinterpret_cast<float*>(smem + L::TILE_BYTES);
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::TILE_BYTES + L::TR_BYTES);
-    uint64_t* empty_bar = full_bar + L::NSTAGE;
-    int* s_flag = reinterpret_cast<int*>(empty_bar + L::NSTAGE);
-    volatile int* s_ready = reinterpret_cast<volatile int*>(s_flag + 1);      // number of grid barriers this CTA has passed
-    float* s_rs = reinterpret_cast<float*>(s_flag + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int nph = cp.n_phases;
-
-    br::launch_dependents();
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < nph; ++i) { br::tma_prefetch_desc(&cp.ph[i].tmW); br::tma_prefetch_desc(&cp.ph[i].tmX); }
-        // full: the W producer's expect_tx covers both halves of a stage (the X producer's load completes the same count);
-        // empty: released by the consumer warpgroup, awaited by both producers
-        for (int s = 0; s < L::NSTAGE; ++s) { br::mbar_init(&full_bar[s], 1); br::mbar_init(&empty_bar[s], 1); }
-        br::mbar_fence_init();
-        *s_ready = 0;
-    }
-    __syncthreads();
-
-    if (warp == 4) {
-        // ---------------- weight producer: never waits for other kernels or phases (weights are constant) ----------------
-        if (lane == 0) {
-            int s = 0; uint32_t ph = 0;
-            for (int pi = 0; pi < nph; ++pi) {
-                const SkParams& p = cp.ph[pi].p;
-                const int u_lo = blockIdx.x * p.chunk, u_hi = min(p.units, u_lo + p.chunk);
-                for (int u = u_lo; u < u_hi; ++u) {
-                    const int tile = u / p.KB, kb = u - tile * p.KB;
-                    br::mbar_wait(&empty_bar[s], ph ^ 1);
-                    br::mbar_expect_tx(&full_bar[s], L::STAGE);
-                    br::tma_load_2d(smem + s * L::STAGE, &cp.ph[pi].tmW, &full_bar[s], kb * BK, tile * BM);
-                    if (++s == L::NSTAGE) { s = 0; ph ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 5) {
-        // ---------------- activation producer: gated by "inputs of phase pi are complete" ----------------
-        if (lane == 0) {
-            br::grid_dep_wait();
-            int s = 0; uint32_t ph = 0;
-            for (int pi = 0; pi < nph; ++pi) {
-                const SkParams& p = cp.ph[pi].p;
-                const int u_lo = blockIdx.x * p.chunk, u_hi = min(p.units, u_lo + p.chunk);
-                if (u_lo < u_hi) while (*s_ready < pi) __nanosleep(32);
-                for (int u = u_lo; u < u_hi; ++u) {
-                    const int tile = u / p.KB, kb = u - tile * p.KB;
-                    br::mbar_wait(&empty_bar[s], ph ^ 1);
-                    br::tma_load_2d(smem + s * L::STAGE + L::A_BYTES, &cp.ph[pi].tmX, &full_bar[s], kb * BK, 0);
-                    if (++s == L::NSTAGE) { s = 0; ph ^= 1; }
-                }
-            }
-        }
-    } else {
-        // ---------------- consumer warpgroup (warps 0..3): wgmma + epilogue ----------------
-        const int lane_grp = warp & 3;
-        const int et = threadIdx.x;
-        CSTAMP(0);
-        br::grid_dep_wait();
-        CSTAMP(1);
-        int s = 0; uint32_t ph = 0;
-        for (int pi = 0; pi < nph; ++pi) {
-            const SkParams& p = cp.ph[pi].p;
-            const int u_lo = blockIdx.x * p.chunk, u_hi = min(p.units, u_lo + p.chunk);
-            CSTAMP(2 + pi * 6);
-            compute_row_rstd(p, et, s_rs, s_rs + 32);      // inputs complete: barrier pi-1 passed
-            int u = u_lo;
-            while (u < u_hi) {
-                const int tile = u / p.KB;
-                const int seg_end = min(u_hi, (tile + 1) * p.KB);
-                const bool whole = (u == tile * p.KB) && (seg_end == (tile + 1) * p.KB);
-                float v[BNX];
-                mma_tile<BNX, BNX>(smem, full_bar, empty_bar, s, ph, seg_end - u, nullptr, s_tr, v);
-                if (u == u_lo) CSTAMP(3 + pi * 6);
-                const int f = tile * BM + lane_grp * 32 + lane;
-                const int part_row = tile * 4 + lane_grp;
-                float res[BNX];
-                load_residual<BNX>(p, f, res);
-                if (whole) {
-                    apply_epilogue<BNX>(p, f, lane, v, res, s_rs, part_row);
-                } else {
-                    const int first_c = (tile * p.KB) / p.chunk, last_c = ((tile + 1) * p.KB - 1) / p.chunk;
-                    const int my_slot = (tile == u_lo / p.KB) ? 0 : 1;
-                    float* mine = p.scratch + (((long long)blockIdx.x * 2 + my_slot) * BNX) * BM + lane_grp * 32 + lane;
-#pragma unroll
-                    for (int r = 0; r < BNX; ++r)
-                        if (r < p.R) __stcg(mine + r * BM, v[r]);
-                    __threadfence();
-                    asm volatile("bar.sync 1, 128;" ::: "memory");
-                    if (et == 0) *s_flag = (atomicAdd(p.counters + tile, 1) == last_c - first_c);
-                    asm volatile("bar.sync 1, 128;" ::: "memory");
-                    if (*s_flag) {
-                        __threadfence();
-#pragma unroll
-                        for (int r = 0; r < BNX; ++r) v[r] = 0.f;
-                        for (int c0 = first_c; c0 <= last_c; c0 += 4) {
-                            float t[4][BNX];
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                const int c = c0 + j;
-                                const int slot = (tile == (c * p.chunk) / p.KB) ? 0 : 1;
-                                const float* src = p.scratch + (((long long)c * 2 + slot) * BNX) * BM + lane_grp * 32 + lane;
-#pragma unroll
-                                for (int r = 0; r < BNX; ++r) t[j][r] = (c <= last_c && r < p.R) ? __ldcg(src + r * BM) : 0.f;
-                            }
-#pragma unroll
-                            for (int j = 0; j < 4; ++j)
-#pragma unroll
-                                for (int r = 0; r < BNX; ++r) v[r] += t[j][r];
-                        }
-                        if (et == 0) p.counters[tile] = 0;
-                        apply_epilogue<BNX>(p, f, lane, v, res, s_rs, part_row);
-                    }
-                    asm volatile("bar.sync 1, 128;" ::: "memory");
-                }
-                u = seg_end;
-            }
-            CSTAMP(4 + pi * 6);
-            if (pi + 1 < nph) {
-                // grid barrier: every CTA's outputs of phase pi are globally visible before anyone loads them as phase pi+1 inputs
-                __threadfence();
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                CSTAMP(5 + pi * 6);
-                if (et == 0) {
-                    atomicAdd(cp.gbar, 1);
-                    const int target = (pi + 1) * (int)gridDim.x;
-                    int seen;
-                    do { asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(seen) : "l"(cp.gbar) : "memory"); } while (seen < target);
-                    *s_ready = pi + 1;
-                }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                CSTAMP(6 + pi * 6);
-            }
-        }
-        // the last CTA to finish re-zeros the barrier words for the next launch (everyone else has left the barrier code)
-        if (et == 0 && nph > 1) {
-            if (atomicAdd(cp.gbar + 1, 1) == (int)gridDim.x - 1) { cp.gbar[0] = 0; cp.gbar[1] = 0; __threadfence(); }
-        }
-    }
-}
-
-template <int BNX>
-int launch_chain(const ChainParams& cp, int grid, cudaStream_t st) {
-    using L = SL<BNX>;
-    auto kern = skinny_chain_kernel<BNX>;
-    static bool done = false;
-    if (!done) { BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL)); done = true; }
-    BR_CHECK_CUDA(br_launch_pdl(kern, dim3(grid), dim3(CHAIN_THREADS), (size_t)L::TOTAL, st, cp));
+    BR_CHECK_CUDA(br_launch_pdl(kern, dim3(grid), dim3(NTHREADS), (size_t)L::TOTAL, st, tw, tx, p));
     return BR_OK;
 }
 
 }  // namespace
 
-static long long* g_sk_dbg = nullptr;
-static int g_sk_dbg_slot = 0;
-
-int br_make_l2_prefetch(const br_l2_prefetch* spec, CUtensorMap* tmap, int* KB, int* units, int* chunk, int* n_chunks, int* a, int* b) {
-    BR_CHECK_ARG(spec->N % 16 == 0 && spec->K % 8 == 0 && spec->ldw % 8 == 0 && spec->unit_lo >= 0, "l2_prefetch: bad weight shape");
-    const int tiles_n = (spec->N + BM - 1) / BM;
-    *KB = (spec->K + BK - 1) / BK; *units = tiles_n * *KB;
-    int grid = *units < br_num_sms() ? *units : br_num_sms();
-    *chunk = (*units + grid - 1) / grid;
-    *n_chunks = (*units + *chunk - 1) / *chunk;
-    *a = spec->unit_lo; *b = spec->unit_hi;
-    return br_make_tmap_2d_bf16(tmap, spec->W, spec->N, spec->K, spec->ldw, BM);
-}
-
 extern "C" {
 
 int64_t br_skinny_scratch_bytes(int max_N) {
-    // partial tiles [n_sms, 2, 32, 128] fp32 | grid-barrier word (16 ints) | one arrival counter per 128-feature tile
-    return (int64_t)br_num_sms() * 2 * 32 * BM * sizeof(float) + 16 * sizeof(int) + (int64_t)(max_N / BM + 2) * sizeof(int);
+    // partial tiles [n_sms, 32, 128] fp32 | one arrival counter per 128-feature tile
+    return (int64_t)br_num_sms() * 32 * BM * sizeof(float) + (int64_t)(max_N / BM + 2) * sizeof(int);
 }
 
 int br_skinny_gemm(const void* X, int64_t ldx, const void* W, int64_t ldw, void* out, int64_t ldo, int R, int N, int K, int mode,
-                   const void* residual, int64_t ldr, void* scratch, void* stream) {
-    return br_skinny_gemm_ex(X, ldx, W, ldw, out, ldo, R, N, K, mode, residual, ldr, scratch, nullptr, 0, nullptr, 0.f, stream);
-}
-
-int br_skinny_gemm_ex(const void* X, int64_t ldx, const void* W, int64_t ldw, void* out, int64_t ldo, int R, int N, int K, int mode,
-                      const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n, float* sumsq_out, float eps,
-                      void* stream) {
-    return br_skinny_gemm_pf(X, ldx, W, ldw, out, ldo, R, N, K, mode, residual, ldr, scratch, sumsq_in, sumsq_in_n, sumsq_out, eps, nullptr, stream);
-}
-
-int br_skinny_grid(int N, int K) {
-    const int units = ((N + BM - 1) / BM) * ((K + BK - 1) / BK);
-    int grid = units < br_num_sms() ? units : br_num_sms();
-    const int chunk = (units + grid - 1) / grid;
-    return (units + chunk - 1) / chunk;
-}
-
-int br_skinny_gemm_pf(const void* X, int64_t ldx, const void* W, int64_t ldw, void* out, int64_t ldo, int R, int N, int K, int mode,
-                      const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n, float* sumsq_out, float eps,
-                      const br_l2_prefetch* prefetch, void* stream) {
-    return br_skinny_gemm_gated(X, ldx, W, ldw, out, ldo, R, N, K, mode, residual, ldr, scratch, sumsq_in, sumsq_in_n, sumsq_out, eps, prefetch, nullptr, stream);
-}
-
-int br_skinny_gemm_gated(const void* X, int64_t ldx, const void* W, int64_t ldw, void* out, int64_t ldo, int R, int N, int K, int mode,
-                         const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n, float* sumsq_out, float eps,
-                         const br_l2_prefetch* prefetch, const br_stream_gate* gate, void* stream) {
+                   const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n, float* sumsq_out, float eps,
+                   void* stream) {
     BR_CHECK_ARG(R >= 1 && R <= 32, "skinny_gemm: R=%d must be in [1, 32]", R);
     BR_CHECK_ARG(N % 16 == 0 && K % 8 == 0 && ldx % 8 == 0 && ldw % 8 == 0, "skinny_gemm: N %% 16, K %% 8, ld %% 8 (N=%d K=%d)", N, K);
     BR_CHECK_ARG(mode >= 0 && mode <= 3 && !(mode == 1 && !residual), "skinny_gemm: bad mode %d", mode);
     BR_CHECK_ARG(scratch != nullptr, "skinny_gemm: scratch (br_skinny_scratch_bytes, zero-initialised once) is required");
     SkParams p;
     p.R = R; p.N = N; p.K = K; p.mode = mode; p.out = out; p.ldo = ldo; p.res = (const bf16*)residual; p.ldr = ldr;
-    p.scratch = (float*)scratch; p.counters = (int*)((float*)scratch + (int64_t)br_num_sms() * 2 * 32 * BM) + 16;
+    p.scratch = (float*)scratch; p.counters = (int*)((float*)scratch + (int64_t)br_num_sms() * 32 * BM);
     p.sumsq_in = sumsq_in; p.sumsq_in_n = sumsq_in_n; p.sumsq_out = sumsq_out; p.eps = eps;
     BR_CHECK_ARG(!(sumsq_out && mode >= 2), "skinny_gemm: sumsq_out only with bf16 outputs (mode 0/1)");
-    p.dbg = g_sk_dbg; p.dbg_slot = g_sk_dbg ? g_sk_dbg_slot++ : 0;
-    p.gate_counter = nullptr; p.gate_epoch = nullptr; p.gate_base = p.gate_per_step = p.gate_signal = 0; p.gate_wait = -1;
-    if (gate && gate->counter) {
-        BR_CHECK_ARG(gate->epoch != nullptr && gate->per_step >= 0, "skinny_gemm: stream gate needs the epoch counter");
-        p.gate_counter = gate->counter; p.gate_epoch = gate->epoch; p.gate_base = gate->epoch_base; p.gate_per_step = gate->per_step;
-        p.gate_wait = gate->wait_prefix; p.gate_signal = gate->signal;
-    }
-    { const char* e = getenv("BR_SKINNY_EVICT_FIRST"); p.w_evict_first = e ? atoi(e) : 1; }
     p.tiles_n = (N + BM - 1) / BM; p.KB = (K + BK - 1) / BK; p.units = p.tiles_n * p.KB;
     int grid = p.units < br_num_sms() ? p.units : br_num_sms();
     p.chunk = (p.units + grid - 1) / grid;
@@ -602,53 +351,9 @@ int br_skinny_gemm_gated(const void* X, int64_t ldx, const void* W, int64_t ldw,
     int rc;
     if ((rc = br_make_tmap_2d_bf16(&tw, W, N, K, ldw, BM))) return rc;
     if ((rc = br_make_tmap_2d_bf16(&tx, X, R, K, ldx, BNX))) return rc;
-    CUtensorMap tp = tw;
-    p.pf_on = 0;
-    if (prefetch && prefetch->W && prefetch->unit_hi > prefetch->unit_lo) {
-        if ((rc = br_make_l2_prefetch(prefetch, &tp, &p.pf.KB, &p.pf.units, &p.pf.chunk, &p.pf.n_chunks, &p.pf.a, &p.pf.b))) return rc;
-        p.pf_on = 1;
-    }
     cudaStream_t st = (cudaStream_t)stream;
-    if (R <= 8) return launch<16, 8>(tw, tx, tp, p, grid, st);
-    return BNX == 16 ? launch<16, 16>(tw, tx, tp, p, grid, st) : launch<32, 32>(tw, tx, tp, p, grid, st);
-}
-
-
-/* profiling aid: [n_launches, 160, 8] int64 %globaltimer stamps of the next br_skinny_gemm launches (NULL disables):
- * 0 kernel entry, 1 dependency wait passed, 2 prologue done (barriers initialised), 3 first accumulator, 4 last partial published, 5 reduction loads done,
- * 6 reducer epilogue done, 7 CTA done */
-int br_skinny_debug(long long* buf) { g_sk_dbg = buf; g_sk_dbg_slot = 0; return BR_OK; }
-
-static long long* g_chain_dbg = nullptr;
-/* profiling aid: [n_sms, 32] int64 %globaltimer stamps of the next chain launches (NULL disables) */
-int br_skinny_chain_debug(long long* buf) { g_chain_dbg = buf; return BR_OK; }
-
-int br_skinny_chain(const br_skinny_phase* phases, int n_phases, int R, float eps, void* scratch, void* stream) {
-    BR_CHECK_ARG(n_phases >= 1 && n_phases <= CHAIN_MAX && R >= 1 && R <= 32 && scratch, "skinny_chain: 1..%d phases, R in [1, 32]", CHAIN_MAX);
-    ChainParams cp;
-    memset(&cp, 0, sizeof(cp));
-    cp.n_phases = n_phases;
-    cp.dbg = g_chain_dbg;
-    const int BNX = R <= 16 ? 16 : 32;
-    const int grid = br_num_sms();                         // every phase uses the full grid: the barrier counts gridDim.x arrivals
-    float* part = (float*)scratch;
-    cp.gbar = (int*)(part + (int64_t)br_num_sms() * 2 * 32 * BM);
-    for (int i = 0; i < n_phases; ++i) {
-        const br_skinny_phase& h = phases[i];
-        BR_CHECK_ARG(h.N % 16 == 0 && h.K % 8 == 0 && h.ldx % 8 == 0 && h.ldw % 8 == 0, "skinny_chain[%d]: N %% 16, K %% 8, ld %% 8", i);
-        BR_CHECK_ARG(h.mode >= 0 && h.mode <= 3 && !(h.mode == 1 && !h.residual) && !(h.sumsq_out && h.mode >= 2), "skinny_chain[%d]: bad mode", i);
-        SkParams& p = cp.ph[i].p;
-        p.R = R; p.N = h.N; p.K = h.K; p.mode = h.mode; p.out = h.out; p.ldo = h.ldo; p.res = (const bf16*)h.residual; p.ldr = h.ldr;
-        p.scratch = part; p.counters = cp.gbar + 16;
-        p.sumsq_in = h.sumsq_in; p.sumsq_in_n = h.sumsq_in_n; p.sumsq_out = h.sumsq_out; p.eps = eps; p.dbg = nullptr; p.dbg_slot = 0; p.w_evict_first = 0;
-        p.tiles_n = (h.N + BM - 1) / BM; p.KB = (h.K + BK - 1) / BK; p.units = p.tiles_n * p.KB;
-        p.chunk = (p.units + grid - 1) / grid;
-        int rc;
-        if ((rc = br_make_tmap_2d_bf16(&cp.ph[i].tmW, h.W, h.N, h.K, h.ldw, BM))) return rc;
-        if ((rc = br_make_tmap_2d_bf16(&cp.ph[i].tmX, h.X, R, h.K, h.ldx, BNX))) return rc;
-    }
-    cudaStream_t st = (cudaStream_t)stream;      // barrier words gbar[0..1] are zero between launches (self-resetting)
-    return BNX == 16 ? launch_chain<16>(cp, grid, st) : launch_chain<32>(cp, grid, st);
+    if (R <= 8) return launch<16, 8>(tw, tx, p, grid, st);
+    return BNX == 16 ? launch<16, 16>(tw, tx, p, grid, st) : launch<32, 32>(tw, tx, p, grid, st);
 }
 
 }  // extern "C"

@@ -9,7 +9,6 @@ prefilled once and share their prompt KV pages.
 from __future__ import annotations
 
 import math
-import os
 from dataclasses import dataclass
 from types import SimpleNamespace
 from typing import List, Optional
@@ -81,20 +80,6 @@ def group_size_from_flags(eq: List[bool]) -> int:
         if B % G == 0 and all(eq[i] for i in range(B) if i % G != 0):
             return G
     return 1
-
-
-def stream_gate_plan(layer_grids, lm_head_grid):
-    """Wait targets of the optional stream gate (br_stream_gate) for one token step.  layer_grids: per layer {w_qkv, w_o, w_gu, w_down: CTAs
-    of that launch}.  Every gated launch adds its grid to one counter when its weights are on chip; a launch waits for the cumulative count
-    of everything launched before it -- except the first qkv GEMM of a step (follows the embedding gather) and every o_proj (follows the
-    attention): HBM idles before those anyway.  Returns ({(layer, name) | "lm_head": target or None}, arrivals per step)."""
-    plan, acc = {}, 0
-    for li, grids in enumerate(layer_grids):
-        for nm in ("w_qkv", "w_o", "w_gu", "w_down"):
-            plan[(li, nm)] = None if (nm == "w_o" or (nm == "w_qkv" and li == 0)) else acc
-            acc += int(grids[nm])
-    plan["lm_head"] = acc
-    return plan, acc + int(lm_head_grid)
 
 
 def plan_pages(plen: List[int], G: int, C: int):
@@ -199,8 +184,7 @@ class RolloutEngine:
         # Static buffers + the captured decode graph are cached per rollout shape: a training run replays the same graph every
         # step (no per-step capture, no graph-pool / allocator churn -- that churn showed up as multi-second host stalls).
         key = (B, G, tuple(plen), C, n_shared, max_pages, n_pages, params.do_sample, params.temperature, params.top_k, params.top_p,
-               params.eos_token_id, params.pad_token_id, id(Wd), bool(use_graph), os.environ.get("BR_DECODE_CHAIN", "0"), os.environ.get("BR_L2PF", "0"), os.environ.get("BR_STREAM_GATE", "0"),
-               os.environ.get("BR_ATTN_SS", ""), os.environ.get("BR_ATTN_SP", ""))
+               params.eos_token_id, params.pad_token_id, id(Wd), bool(use_graph))
         St = self._cached.get(key)
         hit = St is not None
         if not hit:
@@ -247,9 +231,8 @@ class RolloutEngine:
             St.scratch = ops.skinny_scratch(max(cfg.vocab_size, 2 * cfg.intermediate_size), dev)
             # two KV tiles per work item where the co-residency cap allows it: both are fetched before the dependency wait, so the tile loop
             # never waits on DRAM
-            ss_default = min(16, max(8, (n_shared + 1) // 2))
-            splits_shared = min(int(os.environ.get("BR_ATTN_SS", ss_default)), n_shared) if n_shared > 0 else 0
-            splits_private = int(os.environ.get("BR_ATTN_SP", 3)) if n_shared > 0 else 8
+            splits_shared = min(16, max(8, (n_shared + 1) // 2), n_shared) if n_shared > 0 else 0
+            splits_private = 3 if n_shared > 0 else 8
             per_sm = 3                                                                  # CTAs of the fused attention an SM can hold (74 KB each)
             cap = per_sm * torch.cuda.get_device_properties(dev).multi_processor_count      # the fused kernel's merger items need co-residency
             n_items = lambda ss, sp: (R // G) * Hkv * ss + R * Hkv * sp
@@ -267,13 +250,11 @@ class RolloutEngine:
             St.h = torch.empty(R, d, device=dev, dtype=torch.bfloat16)
             n_part_ = ((d + 127) // 128) * 4                                    # partial sum-of-squares rows a d-wide GEMM emits
             St.ssq_a = torch.zeros(n_part_, 32, device=dev, dtype=torch.float32)    # sum x^2 of the residual stream entering attention
-            St.ssq_b = torch.zeros(n_part_, 32, device=dev, dtype=torch.float32)    # ... entering the MLP (see br_skinny_gemm_ex)
+            St.ssq_b = torch.zeros(n_part_, 32, device=dev, dtype=torch.float32)    # ... entering the MLP (see br_skinny_gemm)
             St.ssq_e = torch.zeros(1, 32, device=dev, dtype=torch.float32)          # ... of the embedding row (first layer)
             St.samp_ws = ops.sample_workspace(R, cfg.vocab_size, dev)
-            St.gate = torch.zeros(1, device=dev, dtype=torch.int32)                  # stream-gate arrivals (see br_stream_gate)
             St.graph = None
         else:
-            St.gate.zero_()
             St.tokens.fill_(pad_fill); St.finished.zero_(); St.step.zero_(); St.cur_len.copy_(cur0)
             if params.do_sample:
                 St.uniforms.copy_(uniforms)
@@ -305,77 +286,20 @@ class RolloutEngine:
             St.b_logits = torch.empty(R, cfg.vocab_size, device=dev, dtype=torch.float32)
         b_qkv, b_x2, b_act, b_logits = St.b_qkv, St.b_x2, St.b_act, St.b_logits
 
-        use_chain = os.environ.get("BR_DECODE_CHAIN", "0") == "1"
-
-        def decode_step_chain():
-            # 2 launches per layer: fused attention, then ONE persistent kernel running o_proj (+res) -> gate/up (folded ln2, SwiGLU)
-            # -> down_proj (+res) -> the NEXT layer's qkv projection (folded ln1) / the lm_head, with grid barriers inside.
-            # RMSNorm never launches: its statistics ride along in the GEMM epilogues (sum x^2 partials).
-            ops.embed_gather_sumsq(next_ids, Wd.embed, h, ssq_e)
-            L0 = Wd.layers[0]
-            ops.skinny_gemm(h, L0.w_qkv, scratch, out=b_qkv, sumsq_in=ssq_e, sumsq_in_n=1, eps=eps)
-            nl_ = len(Wd.layers)
-            for li, Lw in enumerate(Wd.layers):
-                ops.decode_attn_fused(b_qkv, Lw.q_norm, Lw.k_norm, kc[li], vc[li], table, cur_len, G, Hq, Hkv, D, n_shared, splits_shared,
-                                      splits_private, theta, eps, ws, attn_out, rope=rope)
-                nxt = (dict(x=h, w=Wd.layers[li + 1].w_qkv, out=b_qkv, mode=0, sumsq_in=ssq_a, sumsq_in_n=n_part) if li + 1 < nl_ else
-                       dict(x=h, w=Wd.lm_head, out=b_logits, mode=3, sumsq_in=ssq_a, sumsq_in_n=n_part))
-                ops.skinny_chain([dict(x=attn_out, w=Lw.w_o, out=b_x2, mode=1, residual=h, sumsq_out=ssq_b),
-                                  dict(x=b_x2, w=Lw.w_gu, out=b_act, mode=2, sumsq_in=ssq_b, sumsq_in_n=n_part),
-                                  dict(x=b_act, w=Lw.w_down, out=h, mode=1, residual=b_x2, sumsq_out=ssq_a),
-                                  nxt], R, scratch, eps=eps)
-            sample(b_logits)
-            ops.decode_advance(step, cur_len)
-
-        # L2 staging plan (BR_L2PF=<fraction>, 0 disables): each launch pulls weight tiles of a LATER GEMM into L2 while HBM would idle
-        # under this launch's dependency waits / reductions.  Of every chunk a consumer CTA streams, tiles [0, 6) arrive through its own
-        # PDL pre-wait ring; a fraction of the rest is staged by the launches before it.
-        pf_frac = float(os.environ.get("BR_L2PF", "0"))
-
-        def stage(w, lo_frac, hi_frac):
-            if pf_frac <= 0.0:
-                return None
-            ch = ops.skinny_chunk_units(w)
-            span = max(0, ch - 6) * pf_frac
-            return (w, 6 + int(span * lo_frac), 6 + int(span * hi_frac))
-
-        # Stream gate (BR_STREAM_GATE=1): a GEMM that becomes resident while its predecessor GEMM is still streaming starts its early weight
-        # loads only when the predecessor's weights are on chip (see br_stream_gate).  `St.gate` counts arrivals; the targets are
-        # cumulative counts within a token step (the graph is replayed per step, the step counter supplies the epoch).
-        use_gate = os.environ.get("BR_STREAM_GATE", "0") not in ("0", "")
-        gate_plan, gate_total = {}, 0
-        if use_gate:
-            gate_plan, gate_total = stream_gate_plan([{nm_: ops.skinny_grid(getattr(Lw_, nm_)) for nm_ in ("w_qkv", "w_o", "w_gu", "w_down")}
-                                                      for Lw_ in Wd.layers], ops.skinny_grid(Wd.lm_head))
-
-        def gate(key):
-            if not use_gate:
-                return None
-            return dict(counter=St.gate, epoch=step, epoch_base=1, per_step=gate_total, wait=gate_plan[key], signal=True)
-
-        def decode_step_5():
+        def decode_step():
             # 5 launches per layer: qkv GEMM (folded ln1), fused attention, o_proj (+res, sum x^2), gate/up GEMM (folded ln2, SwiGLU),
             # down_proj (+res, sum x^2); RMSNorm never launches in the decode loop.
             ops.embed_gather_sumsq(next_ids, Wd.embed, h, ssq_e)
-            nl_ = len(Wd.layers)
             for li, Lw in enumerate(Wd.layers):
-                nxt_w = Wd.layers[li + 1].w_qkv if li + 1 < nl_ else Wd.lm_head
-                ops.skinny_gemm(h, Lw.w_qkv, scratch, out=b_qkv, sumsq_in=ssq_e if li == 0 else ssq_a, sumsq_in_n=1 if li == 0 else n_part, eps=eps,
-                                prefetch=stage(Lw.w_o, 0.0, 1.0), gate=gate((li, "w_qkv")))
+                ops.skinny_gemm(h, Lw.w_qkv, scratch, out=b_qkv, sumsq_in=ssq_e if li == 0 else ssq_a, sumsq_in_n=1 if li == 0 else n_part, eps=eps)
                 ops.decode_attn_fused(b_qkv, Lw.q_norm, Lw.k_norm, kc[li], vc[li], table, cur_len, G, Hq, Hkv, D, n_shared, splits_shared,
-                                      splits_private, theta, eps, ws, attn_out, rope=rope, prefetch=stage(Lw.w_gu, 0.0, 0.65))
-                ops.skinny_gemm(attn_out, Lw.w_o, scratch, mode=1, residual=h, out=b_x2, sumsq_out=ssq_b, prefetch=stage(Lw.w_gu, 0.65, 1.0),
-                                gate=gate((li, "w_o")))
-                ops.skinny_gemm(b_x2, Lw.w_gu, scratch, mode=2, out=b_act, sumsq_in=ssq_b, sumsq_in_n=n_part, eps=eps, prefetch=stage(Lw.w_down, 0.0, 1.0),
-                                gate=gate((li, "w_gu")))
-                ops.skinny_gemm(b_act, Lw.w_down, scratch, mode=1, residual=b_x2, out=h, sumsq_out=ssq_a,
-                                prefetch=stage(nxt_w, 0.0, 1.0) if li + 1 < nl_ else (stage(nxt_w, 0.0, 0.1) if pf_frac > 0 else None),
-                                gate=gate((li, "w_down")))
-            ops.skinny_gemm(h, Wd.lm_head, scratch, mode=3, out=b_logits, sumsq_in=ssq_a, sumsq_in_n=n_part, eps=eps, gate=gate("lm_head"))
+                                      splits_private, theta, eps, ws, attn_out, rope=rope)
+                ops.skinny_gemm(attn_out, Lw.w_o, scratch, mode=1, residual=h, out=b_x2, sumsq_out=ssq_b)
+                ops.skinny_gemm(b_x2, Lw.w_gu, scratch, mode=2, out=b_act, sumsq_in=ssq_b, sumsq_in_n=n_part, eps=eps)
+                ops.skinny_gemm(b_act, Lw.w_down, scratch, mode=1, residual=b_x2, out=h, sumsq_out=ssq_a)
+            ops.skinny_gemm(h, Wd.lm_head, scratch, mode=3, out=b_logits, sumsq_in=ssq_a, sumsq_in_n=n_part, eps=eps)
             sample(b_logits)
             ops.decode_advance(step, cur_len)
-
-        decode_step = decode_step_chain if use_chain else decode_step_5
 
         n_steps = C - 1
         if not hit:
@@ -391,7 +315,6 @@ class RolloutEngine:
                 torch.cuda.current_stream().wait_stream(s)
                 for t, v in zip((tokens, next_ids, finished, step, cur_len), state):
                     t.copy_(v)                                                # the warm-up step is replayed for real below
-                St.gate.zero_()
                 St.graph = torch.cuda.CUDAGraph()
                 n0 = ops.LAUNCHES[0]
                 with torch.cuda.graph(St.graph):

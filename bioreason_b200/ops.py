@@ -5,7 +5,6 @@ are not CUDA tensors -- there is no CPU path.
 """
 from __future__ import annotations
 
-import os
 from typing import Optional
 
 import torch
@@ -239,46 +238,8 @@ def skinny_scratch(max_n: int, device) -> torch.Tensor:
     return torch.zeros(lib().br_skinny_scratch_bytes(max_n), device=device, dtype=torch.uint8)
 
 
-def _l2_prefetch(spec):
-    """(W_later, unit_lo, unit_hi) -> br_l2_prefetch* (or NULL): stage units [lo, hi) of every stream-K chunk of a later decode GEMM into L2."""
-    if spec is None:
-        return ffi.NULL, None
-    w, lo, hi = spec
-    if hi <= lo:
-        return ffi.NULL, None
-    pf = ffi.new("br_l2_prefetch*")
-    pf.W = ptr(w); pf.ldw = _row_major_2d(w); pf.N = w.shape[0]; pf.K = w.shape[1]; pf.unit_lo = int(lo); pf.unit_hi = int(hi)
-    return pf, w
-
-
-def _gate(spec):
-    """dict(counter, epoch, epoch_base, per_step, wait (cumulative arrivals or None), signal (bool)) -> br_stream_gate* (or NULL)."""
-    if spec is None:
-        return ffi.NULL
-    g = ffi.new("br_stream_gate*")
-    g.counter = ptr(spec["counter"], "int32_t*"); g.epoch = ptr(spec["epoch"], "int32_t*")
-    g.epoch_base = int(spec.get("epoch_base", 0)); g.per_step = int(spec["per_step"])
-    g.wait_prefix = -1 if spec.get("wait") is None else int(spec["wait"])
-    g.signal = 1 if spec.get("signal", True) else 0
-    return g
-
-
-def skinny_grid(w) -> int:
-    """CTAs skinny_gemm launches for weight w [N, K]."""
-    return lib().br_skinny_grid(w.shape[0], w.shape[1])
-
-
-def skinny_chunk_units(w) -> int:
-    """16 KB weight tiles one CTA of skinny_gemm streams for weight w [N, K] (the stream-K chunk; mirrors br_skinny_gemm_ex)."""
-    n_sms = torch.cuda.get_device_properties(w.device).multi_processor_count
-    units = ((w.shape[0] + 127) // 128) * ((w.shape[1] + 63) // 64)
-    grid = min(units, n_sms)
-    return (units + grid - 1) // grid
-
-
-def skinny_gemm(x, w, scratch, *, mode=0, residual=None, out=None, sumsq_in=None, sumsq_in_n=1, sumsq_out=None, eps=0.0, prefetch=None, gate=None):
-    """out[R, N] = x[R, K] @ w[N, K].T for R <= 32 decode rows (optionally with the folded-RMSNorm statistics).
-    prefetch=(W_later, unit_lo, unit_hi): also stage tiles of a later GEMM of the chain into L2 (see br_l2_prefetch)."""
+def skinny_gemm(x, w, scratch, *, mode=0, residual=None, out=None, sumsq_in=None, sumsq_in_n=1, sumsq_out=None, eps=0.0):
+    """out[R, N] = x[R, K] @ w[N, K].T for R <= 32 decode rows (optionally with the folded-RMSNorm statistics)."""
     _need_cuda(x, w)
     R, K = x.shape
     N = w.shape[0]
@@ -287,33 +248,12 @@ def skinny_gemm(x, w, scratch, *, mode=0, residual=None, out=None, sumsq_in=None
             out = torch.empty(R, N, device=x.device, dtype=torch.float32)
         else:
             out = torch.empty(R, N // 2 if mode == 2 else N, device=x.device, dtype=torch.bfloat16)
-    pf, _keep = _l2_prefetch(prefetch)
-    check(lib().br_skinny_gemm_gated(ptr(x), _row_major_2d(x), ptr(w), _row_major_2d(w), ptr(out), _row_major_2d(out), R, N, K, mode,
-                                  ptr(residual), _row_major_2d(residual) if residual is not None else 0, ptr(scratch),
-                                  ptr(sumsq_in, "float*"), int(sumsq_in_n) if sumsq_in is not None else 0, ptr(sumsq_out, "float*"),
-                                  float(eps), pf, _gate(gate), _stream()),
+    check(lib().br_skinny_gemm(ptr(x), _row_major_2d(x), ptr(w), _row_major_2d(w), ptr(out), _row_major_2d(out), R, N, K, mode,
+                               ptr(residual), _row_major_2d(residual) if residual is not None else 0, ptr(scratch),
+                               ptr(sumsq_in, "float*"), int(sumsq_in_n) if sumsq_in is not None else 0, ptr(sumsq_out, "float*"),
+                               float(eps), _stream()),
           "skinny_gemm")
     return out
-
-
-def skinny_chain(phases, R, scratch, eps=0.0):
-    """phases: list of dicts(x, w, out, mode=0, residual=None, sumsq_in=None, sumsq_in_n=1, sumsq_out=None) -- up to 4
-    dependent decode GEMMs in one persistent launch (grid barrier between phases, weights prefetched across it)."""
-    n = len(phases)
-    arr = ffi.new("br_skinny_phase[]", n)
-    keep = []
-    for i, ph in enumerate(phases):
-        x, w, out = ph["x"], ph["w"], ph["out"]
-        a = arr[i]
-        a.X = ptr(x); a.ldx = _row_major_2d(x); a.W = ptr(w); a.ldw = _row_major_2d(w); a.out = ptr(out); a.ldo = _row_major_2d(out)
-        a.N = w.shape[0]; a.K = w.shape[1]; a.mode = ph.get("mode", 0)
-        res = ph.get("residual")
-        a.residual = ptr(res); a.ldr = _row_major_2d(res) if res is not None else 0
-        si = ph.get("sumsq_in")
-        a.sumsq_in = ptr(si, "float*"); a.sumsq_in_n = int(ph.get("sumsq_in_n", 1)) if si is not None else 0
-        a.sumsq_out = ptr(ph.get("sumsq_out"), "float*")
-        keep += [x, w, out, res, si]
-    check(lib().br_skinny_chain(arr, n, R, float(eps), ptr(scratch), _stream()), "skinny_chain")
 
 
 def embed_gather_sumsq(ids, table, out, sumsq):
@@ -329,30 +269,9 @@ def scale_columns_(w, scale):
     return w
 
 
-def decode_rope_append(qkv, n_q, n_kv, head_dim, q_norm_w, k_norm_w, cur_len, page_table, kcache, vcache, theta, eps):
-    check(lib().br_decode_rope_append(ptr(qkv), _row_major_2d(qkv), qkv.shape[0], n_q, n_kv, head_dim, ptr(q_norm_w), ptr(k_norm_w),
-                                      ptr(cur_len, "int32_t*"), ptr(page_table, "int32_t*"), page_table.shape[1], ptr(kcache),
-                                      ptr(vcache), float(theta), float(eps), _stream()), "decode_rope_append")
-
-
 def kv_write_pages(qkv_from_first_token, n_tok, n_q, n_kv, head_dim, pages, kcache, vcache):
     check(lib().br_kv_write_pages(ptr(qkv_from_first_token), _row_major_2d(qkv_from_first_token), n_tok, n_q, n_kv, head_dim,
                                   ptr(pages, "int32_t*"), ptr(kcache), ptr(vcache), _stream()), "kv_write_pages")
-
-
-def decode_attn_workspace(R, n_q, head_dim, n_slots, device):
-    return torch.empty(lib().br_decode_attn_workspace_bytes(R, n_q, head_dim, n_slots), device=device, dtype=torch.uint8)
-
-
-def decode_attn(qkv, kcache, vcache, page_table, cur_len, G, n_q, n_kv, head_dim, n_shared_pages, splits_shared, splits_private,
-                workspace, out, scale=None):
-    R = qkv.shape[0]
-    if scale is None:
-        scale = head_dim ** -0.5
-    check(lib().br_decode_attn(ptr(qkv), _row_major_2d(qkv), ptr(kcache), ptr(vcache), ptr(page_table, "int32_t*"), page_table.shape[1],
-                               ptr(cur_len, "int32_t*"), R, G, n_q, n_kv, head_dim, n_shared_pages, splits_shared, splits_private,
-                               float(scale), ptr(workspace), ptr(out), _row_major_2d(out), _stream()), "decode_attn")
-    return out
 
 
 def decode_fused_workspace(R, n_q, n_kv, head_dim, n_slots, device):
@@ -366,16 +285,15 @@ def rope_table(n_pos, head_dim, theta, device):
 
 
 def decode_attn_fused(qkv_raw, q_norm_w, k_norm_w, kcache, vcache, page_table, cur_len, G, n_q, n_kv, head_dim, n_shared_pages,
-                      splits_shared, splits_private, theta, eps, workspace, out, scale=None, rope=None, prefetch=None):
+                      splits_shared, splits_private, theta, eps, workspace, out, scale=None, rope=None):
     R = qkv_raw.shape[0]
     if scale is None:
         scale = head_dim ** -0.5
-    pf, _keep = _l2_prefetch(prefetch)
-    check(lib().br_decode_attn_fused_pf(ptr(qkv_raw), _row_major_2d(qkv_raw), ptr(q_norm_w), ptr(k_norm_w), ptr(kcache), ptr(vcache),
-                                        ptr(page_table, "int32_t*"), page_table.shape[1], ptr(cur_len, "int32_t*"), R, G, n_q, n_kv,
-                                        head_dim, n_shared_pages, splits_shared, splits_private, float(scale), float(theta), float(eps),
-                                        ptr(rope, "float*"), rope.shape[0] if rope is not None else 0,
-                                        ptr(workspace), ptr(out), _row_major_2d(out), pf, _stream()), "decode_attn_fused")
+    check(lib().br_decode_attn_fused(ptr(qkv_raw), _row_major_2d(qkv_raw), ptr(q_norm_w), ptr(k_norm_w), ptr(kcache), ptr(vcache),
+                                     ptr(page_table, "int32_t*"), page_table.shape[1], ptr(cur_len, "int32_t*"), R, G, n_q, n_kv,
+                                     head_dim, n_shared_pages, splits_shared, splits_private, float(scale), float(theta), float(eps),
+                                     ptr(rope, "float*"), rope.shape[0] if rope is not None else 0,
+                                     ptr(workspace), ptr(out), _row_major_2d(out), _stream()), "decode_attn_fused")
     return out
 
 
@@ -387,7 +305,7 @@ def sample_next(logits, *, temperature=1.0, top_k=20, top_p=1.0, do_sample=True,
                 eos_id=-1, pad_id=0, finished=None, tokens=None, next_ids=None, workspace=None):
     R, V = logits.shape
     assert logits.dtype == torch.float32
-    if workspace is not None and (not do_sample or top_k <= 32) and not os.environ.get("BR_SAMPLER_1STAGE"):
+    if workspace is not None and (not do_sample or top_k <= 32):
         check(lib().br_sample_next_2stage(ptr(logits, "float*"), _row_major_2d(logits), R, V, float(temperature), int(top_k), float(top_p),
                                           1 if do_sample else 0, ptr(uniforms, "float*"), ptr(step, "int32_t*"), int(max_steps), int(eos_id),
                                           int(pad_id), ptr(finished, "int32_t*"), ptr(tokens, "int64_t*"), ptr(next_ids, "int64_t*"),

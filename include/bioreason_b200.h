@@ -124,74 +124,24 @@ int br_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const vo
  * KV cache per layer: K and V are [n_pages, Hkv, 64, head_dim] bf16; page_table int32 [R, max_pages];
  * cur_len int32 [R] = tokens already cached for the row (the position of the token being decoded).
  * ------------------------------------------------------------------------------------------- */
+/* scratch of br_skinny_gemm for weights of up to max_N rows: zero-initialised once (its arrival counters self-reset) */
 int64_t br_skinny_scratch_bytes(int max_N);
 /* out[R, N] = X[R, K] . W[N, K]^T for R <= 32 (HBM-bound weight streaming). mode 0: bf16; 1: bf16(out) + residual;
- * 2: SwiGLU over (8 gate | 8 up) row blocks -> [R, N/2]; 3: fp32.  scratch: zero-initialised once (arrival counters self-reset). */
-int br_skinny_gemm(const void* X, int64_t ldx, const void* W, int64_t ldw, void* out, int64_t ldo, int R, int N, int K, int mode,
-                   const void* residual, int64_t ldr, void* scratch, void* stream);
-/* Same with a folded RMSNorm for the decode step (norm weight pre-multiplied into W's columns by br_scale_columns):
+ * 2: SwiGLU over (8 gate | 8 up) row blocks -> [R, N/2]; 3: fp32.
+ * Folded RMSNorm for the decode step (norm weight pre-multiplied into W's columns by br_scale_columns), both optional (NULL):
  * sumsq_in [sumsq_in_n, 32]: partial sums of x^2 per row; out rows are scaled by rsqrt(sum_i sumsq_in[i, r] / K + eps);
  * sumsq_out [ceil(N/128)*4, 32]: partial sums of the bf16-rounded outputs squared (modes 0/1), one partial row per 32
  * features (so the consumer passes sumsq_in_n = ceil(N/128)*4).  No floating-point atomics: the rollout is reproducible. */
-int br_skinny_gemm_ex(const void* X, int64_t ldx, const void* W, int64_t ldw, void* out, int64_t ldo, int R, int N, int K, int mode,
-                      const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n, float* sumsq_out,
-                      float eps, void* stream);
-/* L2 staging for the decode loop.  The decode step is a chain of small dependent kernels; while one of them waits on its predecessor or
- * reduces partial tiles, HBM idles.  A launch can therefore pull weight tiles of a LATER GEMM of the chain into the 50 MB L2:
- * `W [N, K]` is that GEMM's weight, and of every chunk its CTAs will stream (the stream-K decomposition of br_skinny_gemm_ex) the 16 KB
- * tiles [unit_lo, unit_hi) are prefetched.  Weights are constant during a rollout, so this is safe at any point of the chain. */
-typedef struct br_l2_prefetch { const void* W; int64_t ldw; int32_t N, K; int32_t unit_lo, unit_hi; } br_l2_prefetch;
-int br_skinny_gemm_pf(const void* X, int64_t ldx, const void* W, int64_t ldw, void* out, int64_t ldo, int R, int N, int K, int mode,
-                      const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n, float* sumsq_out,
-                      float eps, const br_l2_prefetch* prefetch, void* stream);
-/* Stream gate for the decode chain.  A decode GEMM that becomes resident early fills its weight ring BEFORE its dependency resolves; if
- * the previous GEMM is still streaming, those loads only take bandwidth away from it (its exchange tail starts later by the same amount).
- * With a gate the early loads start when the previous GEMM's weights have all ARRIVED, i.e. they run under its exchange tail, when HBM
- * would idle.  `counter` (int32, zero at the start of a rollout) counts "my weights are on chip" arrivals, one per CTA of every gated
- * launch; a launch starts prefetching once counter >= (*epoch - epoch_base) * per_step + wait_prefix (wait_prefix < 0: at once).  The
- * gate is a timing hint only: the wait is bounded, and a wrong specification costs time, never correctness. */
-typedef struct br_stream_gate { int32_t* counter; const int32_t* epoch; int32_t epoch_base, per_step, wait_prefix, signal; } br_stream_gate;
-int br_skinny_gemm_gated(const void* X, int64_t ldx, const void* W, int64_t ldw, void* out, int64_t ldo, int R, int N, int K, int mode,
-                         const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n, float* sumsq_out,
-                         float eps, const br_l2_prefetch* prefetch, const br_stream_gate* gate, void* stream);
-/* CTAs br_skinny_gemm launches for a weight [N, K] */
-int br_skinny_grid(int N, int K);
-/* Up to 4 dependent decode GEMMs in ONE persistent launch (e.g. o_proj -> gate/up -> down_proj -> next layer's qkv):
- * phases are separated by a grid-wide barrier inside the kernel and the weight producer prefetches across it, so the
- * HBM stream does not stall at layer boundaries.  Same per-phase semantics as br_skinny_gemm_ex. */
-typedef struct br_skinny_phase {
-    const void* X; int64_t ldx;         /* [R, K] bf16 input (for phases > 0: the output of an earlier phase) */
-    const void* W; int64_t ldw;         /* [N, K] bf16 weight */
-    void* out; int64_t ldo;
-    int32_t N, K, mode;
-    const void* residual; int64_t ldr;
-    const float* sumsq_in; int32_t sumsq_in_n;
-    float* sumsq_out;
-} br_skinny_phase;
-int br_skinny_chain(const br_skinny_phase* phases, int n_phases, int R, float eps, void* scratch, void* stream);
-/* profiling aid: [n_sms, 32] int64 %globaltimer stamps (per CTA: start, dep-wait, then per phase: begin, first accumulator,
- * tiles done, barrier arrive, barrier pass) written by the next br_skinny_chain launches; NULL disables */
-int br_skinny_chain_debug(long long* buf);
-/* profiling aid for br_skinny_gemm(_ex): [n_launches, 160, 8] int64 %globaltimer stamps per CTA of the following launches
- * (kernel entry, dependency wait passed, prologue done, first accumulator, partial published, reduction loads, reducer epilogue, done) */
-int br_skinny_debug(long long* buf);
+int br_skinny_gemm(const void* X, int64_t ldx, const void* W, int64_t ldw, void* out, int64_t ldo, int R, int N, int K, int mode,
+                   const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n, float* sumsq_out,
+                   float eps, void* stream);
 int br_embed_gather_sumsq(const int64_t* ids, const void* table, int64_t ldt, int64_t vocab, void* out, int64_t ldo, int M, int d,
                           float* sumsq, void* stream);
 /* W[n, k] *= scale[k] in place (bf16) */
 int br_scale_columns(void* W, int64_t ld, int64_t N, int K, const void* scale, void* stream);
-/* per-head q/k RMSNorm + RoPE at position cur_len[r]; K and V of the new token go into the row's page, Q stays in qkv */
-int br_decode_rope_append(void* qkv, int64_t ld, int R, int n_q_heads, int n_kv_heads, int head_dim, const void* q_norm_w,
-                          const void* k_norm_w, const int32_t* cur_len, const int32_t* page_table, int max_pages,
-                          void* kcache, void* vcache, float theta, float eps, void* stream);
 /* prefill: copy roped K / V of tokens [0, n_tok) of one prompt row (qkv points at its first real token) into pages[] */
 int br_kv_write_pages(const void* qkv, int64_t ld, int n_tok, int n_q_heads, int n_kv_heads, int head_dim, const int32_t* pages,
                       void* kcache, void* vcache, void* stream);
-int64_t br_decode_attn_workspace_bytes(int R, int n_q_heads, int head_dim, int n_slots);
-/* one decode-attention step; rows are R/G groups whose first n_shared_pages table entries are identical (prefix sharing:
- * the shared pass reads each prompt K/V tile once per group). n_slots = splits_shared (if used) + splits_private. */
-int br_decode_attn(const void* qkv, int64_t ld, const void* kcache, const void* vcache, const int32_t* page_table, int max_pages,
-                   const int32_t* cur_len, int R, int G, int n_q_heads, int n_kv_heads, int head_dim, int n_shared_pages,
-                   int splits_shared, int splits_private, float scale, void* workspace, void* out, int64_t ldo, void* stream);
 /* temperature -> top-k -> top-p -> inverse-CDF draw with uniforms[step*R + r] (or argmax when !do_sample); finished rows
  * emit pad_id; writes tokens[r, step] (int64 [R, max_steps]) and next_ids[r]; eos_id < 0 disables EOS. */
 int br_sample_next(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
@@ -205,25 +155,20 @@ int br_sample_next_2stage(const float* logits, int64_t ld, int R, int V, float t
                           int32_t* finished, int64_t* tokens, int64_t* next_ids, void* workspace, void* stream);
 int br_decode_advance(int32_t* step, int32_t* cur_len, int R, void* stream);
 
-/* Fused decode attention (one launch per layer per step): per-head q/k RMSNorm + RoPE at cur_len[r], K/V append to the
- * row's page, prefix-shared + private paged attention, split merge.  qkv_raw is the un-normalised fused projection of
- * the new tokens.  workspace: br_decode_fused_workspace_bytes, zero-initialised once (arrival counters are self-resetting). */
+/* Decode attention, one launch per layer per step: per-head q/k RMSNorm + RoPE at cur_len[r], K/V append to the row's page,
+ * paged attention and split merge.  qkv_raw is the un-normalised fused projection of the new tokens.  Rows are R/G groups whose
+ * first n_shared_pages table entries are identical (prefix sharing: the shared pass reads each prompt K/V tile once per group);
+ * G * n_q_heads/n_kv_heads <= 32.  splits_shared + splits_private <= 32 partial slots per head.  rope_table (br_rope_table,
+ * covering every position of the rollout) is required.  workspace: br_decode_fused_workspace_bytes, zero-initialised once
+ * (arrival counters are self-resetting). */
 int64_t br_decode_fused_workspace_bytes(int R, int n_q_heads, int n_kv_heads, int head_dim, int n_slots);
 int br_decode_attn_fused(const void* qkv_raw, int64_t ld, const void* q_norm_w, const void* k_norm_w, void* kcache, void* vcache,
                          const int32_t* page_table, int max_pages, const int32_t* cur_len, int R, int G, int n_q_heads,
                          int n_kv_heads, int head_dim, int n_shared_pages, int splits_shared, int splits_private, float scale,
                          float theta, float eps, const float* rope_table, int rope_n_pos, void* workspace, void* out, int64_t ldo,
                          void* stream);
-/* same, plus L2 staging of a later GEMM's weight tiles from this (HBM-light) launch; see br_l2_prefetch */
-int br_decode_attn_fused_pf(const void* qkv_raw, int64_t ld, const void* q_norm_w, const void* k_norm_w, void* kcache, void* vcache,
-                            const int32_t* page_table, int max_pages, const int32_t* cur_len, int R, int G, int n_q_heads, int n_kv_heads,
-                            int head_dim, int n_shared_pages, int splits_shared, int splits_private, float scale, float theta, float eps,
-                            const float* rope_table, int rope_n_pos, void* workspace, void* out, int64_t ldo, const br_l2_prefetch* prefetch,
-                            void* stream);
 /* rope_table [n_pos, head_dim/2, 2] f32 = (cos, sin) rounded to bf16 precision (HF builds its tables in the model dtype);
- * optional input of br_decode_attn_fused: removes powf/sincosf from the decode loop. */
-/* profiling aid: per-item phase timestamps ([items, 16] int64, %globaltimer ns) for the next fused-attention launches */
-int br_decode_attn_fused_debug(long long* buf);
+ * input of br_decode_attn_fused: removes powf/sincosf from the decode loop. */
 int br_rope_table(float* out, int n_pos, int head_dim, float theta, void* stream);
 
 /* ---------------------------------------------------------------------------------------------

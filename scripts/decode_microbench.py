@@ -68,28 +68,12 @@ qkv = torch.randn(R, (Hq + 2 * Hkv) * D, device=dev).to(bf)
 qn = torch.ones(D, device=dev).to(bf); kn = torch.ones(D, device=dev).to(bf)
 cur = torch.full((R,), T, dtype=torch.int32, device=dev)
 rope = ops.rope_table(T + 8, D, 1e6, dev)
-for ss, sp in ((8, 2), (14, 3), (16, 2), (28, 3), (28, 2), (4, 1)):
+for ss, sp in ((8, 2), (14, 3), (16, 2), (28, 2), (4, 1)):       # <= 3 work items per SM on a 132-SM H100
     wsf = ops.decode_fused_workspace(R, Hq, Hkv, D, ss + sp, dev)
     out = torch.empty(R, Hq * D, device=dev, dtype=bf)
     us = timed_graph(lambda: ops.decode_attn_fused(qkv, qn, kn, kc, vc, table, cur, G, Hq, Hkv, D, n_shared, ss, sp, 1e6, 1e-6, wsf, out, rope=rope), inner=4)
     print(f"decode_attn_fused ctx={T} splits=({ss},{sp}): {us:8.2f} us")
     res[f"attn_fused_{ss}_{sp}"] = (us, 0)
-
-# phase timestamps of one fused-attention launch
-from bioreason_b200._lib import lib as _lib, ffi as _ffi
-items = 64 + 128
-dbg = torch.zeros(items, 16, dtype=torch.int64, device=dev)
-_lib().br_decode_attn_fused_debug(_ffi.cast("long long*", dbg.data_ptr()))
-wsf = ops.decode_fused_workspace(R, Hq, Hkv, D, 10, dev); out = torch.empty(R, Hq * D, device=dev, dtype=bf)
-for _ in range(3):
-    ops.decode_attn_fused(qkv, qn, kn, kc, vc, table, cur, G, Hq, Hkv, D, n_shared, 8, 2, 1e6, 1e-6, wsf, out, rope=rope)
-torch.cuda.synchronize()
-_lib().br_decode_attn_fused_debug(_ffi.NULL)
-t = dbg.double().cpu(); t0 = t[:, 0].min()
-rel = (t - t0) / 1e3
-names = ["start", "dep_wait", "q_prep", "tile0", "tiles", "partials", "counter", "end", "q_loaded", "q_roped"]
-for lab, sl in (("shared", slice(0, 64)), ("private", slice(64, 192))):
-    print(f"fused attention phases ({lab}, us since first CTA start): " + "  ".join(f"{n}={rel[sl, i].mean():.1f}/{rel[sl, i].max():.1f}" for i, n in enumerate(names)))
 
 # sampler
 logits = torch.randn(R, V, device=dev)
@@ -118,47 +102,16 @@ x0 = torch.randn(R, d, device=dev).to(bf)
 cur.fill_(T); step.zero_()          # decode_advance above moved them
 n_part = ((d + 127) // 128) * 4
 ssa = torch.ones(n_part, 32, device=dev); ssb = torch.ones(n_part, 32, device=dev)
-wsf = ops.decode_fused_workspace(R, Hq, Hkv, D, 10, dev)
 attn_out = torch.empty(R, Hq * D, device=dev, dtype=bf)
-SS_, SP_ = int(os.environ.get("BR_ATTN_SS", 8)), int(os.environ.get("BR_ATTN_SP", 2))
+SS_, SP_ = 8, 2
 wsf = ops.decode_fused_workspace(R, Hq, Hkv, D, SS_ + SP_, dev)
-for frac in (0.0, 0.5, 1.0):
-    def stage(w, lo, hi):
-        if frac <= 0:
-            return None
-        span = max(0, ops.skinny_chunk_units(w) - 6) * frac
-        return (w, 6 + int(span * lo), 6 + int(span * hi))
-    def chain():
-        x = x0
-        for i, w in enumerate(ws_l):
-            wn = ws_l[(i + 1) % NL]["qkv"]
-            q = ops.skinny_gemm(x, w["qkv"], scratch, sumsq_in=ssa, sumsq_in_n=n_part, eps=1e-6, prefetch=stage(w["o"], 0, 1))
-            ops.decode_attn_fused(q, qn, kn, kc, vc, table, cur, G, Hq, Hkv, D, n_shared, SS_, SP_, 1e6, 1e-6, wsf, attn_out, rope=rope, prefetch=stage(w["gu"], 0, 0.65))
-            x2 = ops.skinny_gemm(attn_out, w["o"], scratch, mode=1, residual=x, sumsq_out=ssb, prefetch=stage(w["gu"], 0.65, 1))
-            a = ops.skinny_gemm(x2, w["gu"], scratch, mode=2, sumsq_in=ssb, sumsq_in_n=n_part, eps=1e-6, prefetch=stage(w["down"], 0, 1))
-            x = ops.skinny_gemm(a, w["down"], scratch, mode=1, residual=x2, sumsq_out=ssa, prefetch=stage(wn, 0, 1))
-    us = timed_graph(chain) / NL
-    print(f"layer chain (5 launches, splits {SS_},{SP_}, L2 staging {frac:.1f}): {us:8.2f} us per layer  -> {36 * us / 1e3:.3f} ms per token (36 layers)   PDL={'off' if os.environ.get('BR_NO_PDL') else 'on'}")
-
-# ---- the production layout: fused attention + ONE persistent chain kernel (o -> gate/up -> down -> next qkv) per layer
-b_qkv = torch.empty(R, (Hq + 2 * Hkv) * D, device=dev, dtype=bf); b_x2 = torch.empty(R, d, device=dev, dtype=bf)
-b_act = torch.empty(R, F, device=dev, dtype=bf); hbuf = x0.clone()
-wsf2 = ops.decode_fused_workspace(R, Hq, Hkv, D, 10, dev)
-def chain2():
-    for i, w in enumerate(ws_l):
-        ops.decode_attn_fused(b_qkv, qn, kn, kc, vc, table, cur, G, Hq, Hkv, D, n_shared, 8, 2, 1e6, 1e-6, wsf2, attn_out, rope=rope)
-        ops.skinny_chain([dict(x=attn_out, w=w["o"], out=b_x2, mode=1, residual=hbuf, sumsq_out=ssb),
-                          dict(x=b_x2, w=w["gu"], out=b_act, mode=2, sumsq_in=ssb, sumsq_in_n=n_part),
-                          dict(x=b_act, w=w["down"], out=hbuf, mode=1, residual=b_x2, sumsq_out=ssa),
-                          dict(x=hbuf, w=ws_l[(i + 1) % NL]["qkv"], out=b_qkv, mode=0, sumsq_in=ssa, sumsq_in_n=n_part)], R, scratch, eps=1e-6)
-us = timed_graph(chain2) / NL
-print(f"layer = fused attention + persistent 4-phase GEMM chain: {us:8.2f} us per layer -> {36 * us / 1e3:.3f} ms per token; "
-      f"weight bytes {sum(v.numel() for v in ws_l[0].values()) * 2 / 1e6:.1f} MB -> {sum(v.numel() for v in ws_l[0].values()) * 2 / (us * 1e-6) / 1e9:.0f} GB/s incl. attention")
-def chain_only():
-    for i, w in enumerate(ws_l):
-        ops.skinny_chain([dict(x=attn_out, w=w["o"], out=b_x2, mode=1, residual=hbuf, sumsq_out=ssb),
-                          dict(x=b_x2, w=w["gu"], out=b_act, mode=2, sumsq_in=ssb, sumsq_in_n=n_part),
-                          dict(x=b_act, w=w["down"], out=hbuf, mode=1, residual=b_x2, sumsq_out=ssa),
-                          dict(x=hbuf, w=ws_l[(i + 1) % NL]["qkv"], out=b_qkv, mode=0, sumsq_in=ssa, sumsq_in_n=n_part)], R, scratch, eps=1e-6)
-us = timed_graph(chain_only) / NL
-print(f"persistent 4-phase GEMM chain alone: {us:8.2f} us per layer  ({sum(v.numel() for v in ws_l[0].values()) * 2 / (us * 1e-6) / 1e9:.0f} GB/s)")
+def chain():
+    x = x0
+    for w in ws_l:
+        q = ops.skinny_gemm(x, w["qkv"], scratch, sumsq_in=ssa, sumsq_in_n=n_part, eps=1e-6)
+        ops.decode_attn_fused(q, qn, kn, kc, vc, table, cur, G, Hq, Hkv, D, n_shared, SS_, SP_, 1e6, 1e-6, wsf, attn_out, rope=rope)
+        x2 = ops.skinny_gemm(attn_out, w["o"], scratch, mode=1, residual=x, sumsq_out=ssb)
+        a = ops.skinny_gemm(x2, w["gu"], scratch, mode=2, sumsq_in=ssb, sumsq_in_n=n_part, eps=1e-6)
+        x = ops.skinny_gemm(a, w["down"], scratch, mode=1, residual=x2, sumsq_out=ssa)
+us = timed_graph(chain) / NL
+print(f"layer chain (5 launches, splits {SS_},{SP_}): {us:8.2f} us per layer  -> {36 * us / 1e3:.3f} ms per token (36 layers)   PDL={'off' if os.environ.get('BR_NO_PDL') else 'on'}")

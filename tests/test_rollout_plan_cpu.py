@@ -63,18 +63,3 @@ def test_sampling_params_from_hf_kwargs():
     with pytest.raises(NotImplementedError, match="distinct eos_token_id"):                                        # never silently keep eos[0]
         SamplingParams.from_hf_kwargs(cfg, dict(eos_token_id=[11, 12]))
 
-
-def test_stream_gate_plan():
-    """Targets of the optional stream gate: cumulative arrivals of everything launched earlier in the token step; the first qkv GEMM and
-    every o_proj start unguarded; the per-step total is what the epoch multiplies."""
-    from bioreason_b200.generation import stream_gate_plan
-    g = dict(w_qkv=148, w_o=143, w_gu=145, w_down=145)
-    plan, total = stream_gate_plan([g, g, g], 148)
-    per_layer = sum(g.values())
-    assert total == 3 * per_layer + 148
-    assert plan[(0, "w_qkv")] is None and all(plan[(li, "w_o")] is None for li in range(3))
-    assert plan[(0, "w_gu")] == 148 + 143 and plan[(0, "w_down")] == 148 + 143 + 145
-    assert plan[(1, "w_qkv")] == per_layer and plan[(2, "w_down")] == 2 * per_layer + 148 + 143 + 145
-    assert plan["lm_head"] == 3 * per_layer
-    waits = [v for v in plan.values() if v is not None]
-    assert waits == sorted(waits) and max(waits) < total

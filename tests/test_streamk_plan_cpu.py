@@ -1,6 +1,6 @@
-"""Pure-Python model of the stream-K decomposition arithmetic in csrc/decode_gemm_tc5.cu (skinny_tc5_kernel /
-skinny_chain_kernel): which CTA contributes to which feature tile, which of its two scratch slots it uses, and which CTAs the
-reducing CTA reads -- the invariants the deterministic fixed-order reduction relies on."""
+"""Pure-Python model of the stream-K decomposition arithmetic in csrc/decode_gemm_tc5.cu (skinny_tc5_kernel): which CTA
+contributes to which feature tile, which partial tile it publishes to its one scratch slot, and which CTAs the reducing CTA
+reads -- the invariants the deterministic fixed-order reduction relies on."""
 import math
 
 import pytest
@@ -18,15 +18,14 @@ def plan(N, K, n_sms=148):
 
 
 def segments(c, KB, units, chunk):
-    """(tile, k_lo, k_hi, whole, slot) for every segment CTA c processes, in order (mirrors the epilogue loop)."""
+    """(tile, k_lo, k_hi, whole) for every segment CTA c processes, in order (mirrors the epilogue loop)."""
     u_lo, u_hi = c * chunk, min(units, (c + 1) * chunk)
     u, out = u_lo, []
     while u < u_hi:
         tile = u // KB
         seg_end = min(u_hi, (tile + 1) * KB)
         whole = (u == tile * KB) and (seg_end == (tile + 1) * KB)
-        slot = 0 if tile == u_lo // KB else 1
-        out.append((tile, u - tile * KB, seg_end - tile * KB, whole, slot))
+        out.append((tile, u - tile * KB, seg_end - tile * KB, whole))
         u = seg_end
     return out
 
@@ -41,11 +40,14 @@ def test_streamk_invariants(N, K, n_sms):
     covered = {}
     for c in range(grid):
         segs = segments(c, KB, units, chunk)
-        partial = [s for s in segs if not s[3]]
-        assert len(partial) <= 2                                                 # two scratch slots per CTA suffice
-        assert len({s[4] for s in partial}) == len(partial)                      # ... and they never collide
-        for (tile, lo, hi, whole, slot) in segs:
-            covered.setdefault(tile, []).append((lo, hi, c, whole, slot))
+        for i, (tile, lo, hi, whole) in enumerate(segs):
+            if not whole:
+                first_c = (tile * KB) // chunk
+                if c == first_c:
+                    assert i == len(segs) - 1                                    # the reducer meets the tile as its last segment
+                else:                                                            # a publisher's partial starts its chunk:
+                    assert i == 0                                                # one scratch slot per CTA suffices
+            covered.setdefault(tile, []).append((lo, hi, c, whole))
     assert sorted(covered) == list(range(tiles))
     for tile, parts in covered.items():
         parts.sort()
@@ -56,7 +58,5 @@ def test_streamk_invariants(N, K, n_sms):
             assert parts[0][3]                                                    # single owner -> direct epilogue, no scratch
         else:
             assert not any(p[3] for p in parts)
-            for (lo, hi, c, whole, slot) in parts:                                # the slot the reducer reads == the slot the writer used
-                assert slot == (0 if tile == (c * chunk) // KB else 1)
         # arrival counter: the last arriver sees (contributors - 1)
         assert last_c - first_c == len(parts) - 1
