@@ -134,6 +134,20 @@ __device__ __forceinline__ float2 unpack_bf16(uint32_t v) {
     return __bfloat1622float2(t);
 }
 
+// ---------------- counter-based random numbers ----------------
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011): ten rounds of two 32x32->64-bit
+// multiplies with a Weyl-sequence key schedule.  Stateless: the same (counter, key) gives the same 128 bits on any thread.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+    for (int i = 0; i < 10; ++i) {
+        if (i) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+        const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+    }
+    return c;
+}
+
 }  // namespace br
 #endif
 

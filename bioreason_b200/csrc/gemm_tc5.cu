@@ -8,10 +8,14 @@
 //   warps 0..7  two consumer warpgroups: each issues wgmma.mma_async m64n128k16 for its 64 rows of the 128 x 128 tile (one
 //                                wgmma group kept in flight; a stage goes back to the producer as soon as its products retire),
 //                                then runs the fused epilogue straight from the register fragment
+// LoRA dropout (MASK): the second K segment u . A of the dX GEMM is formed one projection (r-wide K block) at a time in a temporary
+// accumulator, multiplied by that projection's counter-based mask and 1 / (1 - p_eff) in registers, and added to the main accumulator
+// before the usual epilogue (one rounding, no extra HBM traffic).
 // Epilogue modes: plain (+bias, +residual, gated-SiLU on interleaved column pairs, fp32/bf16 out, row scatter),
 // online log-sum-exp partials + target-logit gather (lm_head; logits never reach HBM), and softmax-gradient tiles.
 #include "br_common.cuh"
 #include "../../include/bioreason_b200.h"
+#include "lora_dropout.cuh"
 #include "wgmma.cuh"
 
 namespace {
@@ -40,6 +44,7 @@ struct GemmParams {
     const float* lse; const float* gscale;        // [M]
     int n_tiles_m, n_tiles_n;
     int group_m;             // m-blocks per raster group (see tile_coords)
+    br::DropParams drop;     // MASK: dropout of the second segment's projections
 };
 
 struct SmemLayout {
@@ -65,7 +70,46 @@ __device__ __forceinline__ void tile_coords(int tile, int ntm, int ntn, int GROU
 
 __device__ __forceinline__ float rbf(float x) { return __bfloat162float(__float2bfloat16(x)); }
 
-template <int MODE>
+// One BK block of the LoRA segment under dropout: for each projection whose r-wide K slice lies in the block, tmp = u_j . A_j (its k16
+// steps), then acc += m_j * inv_keep * tmp over the thread's fragment.  Retires every outstanding wgmma of the tile first.
+__device__ __forceinline__ void masked_segment(float (&acc)[BN / 2], uint64_t adesc, uint64_t bdesc, int k0, int mb, int nb, int wg,
+                                               const GemmParams& p) {
+    const int lane = threadIdx.x & 31, q = lane & 3;
+    const long long grow = p.drop.row0 + mb * BM + wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+    const int cg0 = (nb * BN) >> 3;
+    br::wg_wait<0>();
+    br::wg_fence_operand(acc);
+    for (int kk = 0; kk < BK / 16;) {
+        const int kc = k0 + 16 * kk;
+        if (kc >= p.K2) break;
+        const int jb = kc / p.drop.r;
+        const int nk = min(p.drop.r - (kc - jb * p.drop.r), BK - 16 * kk) >> 4;     // k16 steps of projection jb in this block
+        float tmp[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) tmp[i] = 0.f;
+        br::wg_fence();
+        for (int t = 0; t < nk; ++t) br::wgmma_ss<BN>(tmp, adesc + 2 * (kk + t), bdesc + 2 * (kk + t), 1);
+        br::wg_commit();
+        br::wg_wait<0>();
+        br::wg_fence_operand(tmp);
+        const int j = p.drop.proj + jb;
+#pragma unroll
+        for (int set = 0; set < BN / 16; ++set) {                   // 2 rows x BN / 8 column groups = BN / 4 groups, 4 per set
+            // groups g = 0..3 of this set: column group 2 set + (g >> 1), row + 8 (g & 1); lane q draws group q
+            uint32_t w[4];
+            br::quad_words(br::drop_group(p.drop, grow + 8 * (q & 1), cg0 + 2 * set + (q >> 1), j), w);
+#pragma unroll
+            for (int g = 0; g < 4; ++g) {
+                const int e = 4 * (2 * set + (g >> 1)) + 2 * (g & 1);
+                acc[e] += br::keep_lo(w[g], p.drop.T) ? tmp[e] * p.drop.inv_keep : 0.f;
+                acc[e + 1] += br::keep_hi(w[g], p.drop.T) ? tmp[e + 1] * p.drop.inv_keep : 0.f;
+            }
+        }
+        kk += nk;
+    }
+}
+
+template <int MODE, bool MASK>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
@@ -131,6 +175,15 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             const uint32_t sa = br::smem_u32(smem + s * L::STAGE_BYTES);
             const uint64_t adesc = br::wg_desc_k(sa + wg * 64 * 128);
             const uint64_t bdesc = br::wg_desc_k(sa + L::A_BYTES);
+            if constexpr (MASK) {
+                if (kb >= kb1) {
+                    masked_segment(acc, adesc, bdesc, (kb - kb1) * BK, mb, nb, wg, p);
+                    if (wt == 0) br::mbar_arrive(&empty_bar[prev]);       // masked_segment retired every product: release the previous stage
+                    prev = s;
+                    if (++s == L::NSTAGE) { s = 0; ph ^= 1; }
+                    continue;
+                }
+            }
             br::wg_fence();
 #pragma unroll
             for (int k = 0; k < BK / 16; ++k) br::wgmma_ss<BN>(acc, adesc + 2 * k, bdesc + 2 * k, 1);
@@ -293,9 +346,9 @@ PFN_encodeTiled get_encode() {
     return fn;
 }
 
-template <int MODE>
+template <int MODE, bool MASK = false>
 int launch(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& a2, const CUtensorMap& b2, const GemmParams& p, cudaStream_t st) {
-    auto kern = gemm_tc5_kernel<MODE>;
+    auto kern = gemm_tc5_kernel<MODE, MASK>;
     static bool attr_set = false;
     if (!attr_set) {
         BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemLayout::TOTAL));
@@ -309,7 +362,7 @@ int launch(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& a2, co
 }
 
 int run_gemm(int mode, const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, const void* A2, int64_t lda2,
-             const void* B2, int64_t ldb2, int K2, GemmParams& p, cudaStream_t st) {
+             const void* B2, int64_t ldb2, int K2, GemmParams& p, cudaStream_t st, bool masked = false) {
     BR_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
     BR_CHECK_ARG(N % 8 == 0 && K % 8 == 0 && lda % 8 == 0 && ldb % 8 == 0, "gemm: N, K, lda, ldb must be multiples of 8");
     BR_CHECK_ARG(((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0), "gemm: operands must be 16-byte aligned");
@@ -332,6 +385,7 @@ int run_gemm(int mode, const void* A, int64_t lda, const void* B, int64_t ldb, i
         if ((rc = br_make_tmap_2d_bf16(&ta2, A2, M, K2, lda2, BM))) return rc;
         if ((rc = br_make_tmap_2d_bf16(&tb2, B2, N, K2, ldb2, BN))) return rc;
     } else { ta2 = ta; tb2 = tb; }
+    if (masked) return launch<MODE_STD, true>(ta, tb, ta2, tb2, p, st);
     if (mode == MODE_STD) return launch<MODE_STD>(ta, tb, ta2, tb2, p, st);
     if (mode == MODE_LSE) return launch<MODE_LSE>(ta, tb, ta2, tb2, p, st);
     return launch<MODE_DLOGITS>(ta, tb, ta2, tb2, p, st);
@@ -364,6 +418,7 @@ int br_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ldb, void* D
     memset(&p, 0, sizeof(p));
     p.D = D; p.ldd = (int)ldd; p.alpha = 1.f;
     const void *A2 = nullptr, *B2 = nullptr; int64_t lda2 = 0, ldb2 = 0; int K2 = 0;
+    bool masked = false;
     if (e) {
         p.bias = e->bias; p.bias_f32 = e->bias_dtype == BR_F32;
         p.residual = reinterpret_cast<const bf16*>(e->residual); p.ldr = e->ldr;
@@ -372,9 +427,19 @@ int br_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ldb, void* D
         A2 = e->A2; B2 = e->B2; lda2 = e->lda2; ldb2 = e->ldb2; K2 = e->K2;
         BR_CHECK_ARG(!(p.act == 1 && (p.out_f32 || p.residual)), "gemm: gated-SiLU epilogue writes bf16 without residual");
         BR_CHECK_ARG(!(p.act == 1 && N % 16 != 0), "gemm: gated-SiLU epilogue needs N %% 16 == 0");
+        if (e->lora_dropout) {
+            int rc;
+            if ((rc = br::check_drop(e->lora_dropout, "gemm"))) return rc;
+            const int r = e->lora_dropout->r;
+            BR_CHECK_ARG(A2 && B2 && r % 16 == 0 && r > 0 && K2 % r == 0 && e->lora_dropout->proj + K2 / r <= 8,
+                         "gemm: masked LoRA segment needs A2/B2 with K2 = n_proj * r, r %% 16 == 0 (K2=%d r=%d)", K2, r);
+            BR_CHECK_ARG(!p.row_map, "gemm: masked LoRA segment indexes mask rows by input row; no row_map");
+            p.drop = br::drop_params(*e->lora_dropout);
+            masked = true;
+        }
     }
     BR_CHECK_ARG(ldd % 8 == 0 && (uintptr_t)D % 16 == 0, "gemm: D must be 16-byte aligned with ldd %% 8 == 0");
-    return run_gemm(MODE_STD, A, lda, B, ldb, M, N, K, A2, lda2, B2, ldb2, K2, p, (cudaStream_t)stream);
+    return run_gemm(MODE_STD, A, lda, B, ldb, M, N, K, A2, lda2, B2, ldb2, K2, p, (cudaStream_t)stream, masked);
 }
 
 int64_t br_lmhead_workspace_bytes(int M, int V) {

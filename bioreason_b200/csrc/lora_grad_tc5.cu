@@ -7,8 +7,12 @@
 // block each adapter owns (q rows x its r columns, ...), so 14 launches per decoder layer become 8.
 // Split-K over the token dimension fills the SMs for narrow outputs; partial tiles are exchanged through a workspace and summed
 // by the split-0 CTA in ascending split order (release/acquire counter, no floating-point atomics): gradients are bit-reproducible.
+// With LoRA dropout (MASK, dA = inv_keep * u^T (x . m)): the MN-major `big` tile is loaded into register fragments (ldmatrix.trans),
+// ANDed with the counter-based mask and fed to the register-A wgmma; each lane draws one (token, 8-feature) group per k16 step and the
+// warp trades the 16-bit draws through 512 bytes of shared memory.
 #include "br_common.cuh"
 #include "../../include/bioreason_b200.h"
+#include "lora_dropout.cuh"
 #include "wgmma.cuh"
 
 namespace {
@@ -26,9 +30,30 @@ struct TnParams {
                                                // 2: gate/up interleave: product row p = block of 16 = 8 gate | 8 up -> dst rows (p/16)*8 + p%8
     Seg seg[3]; int n_seg;
     float* ws; int* counters;
+    br::DropParams drop;                       // MASK only
 };
 
-template <int NPAD>
+// Masked A fragment (features 16 w.. of one 64-feature block x tokens t0 + 0..15): a[i] = feature + 8 (i & 1), tokens + 8 (i >> 1) + 2q, +1
+__device__ __forceinline__ void masked_big_frag(uint32_t (&a)[4], uint32_t blk, int kk, long long tok0, int feat0, const br::DropParams& d,
+                                                uint4* xbuf) {
+    const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3, mi = lane >> 3;
+    const int tok = kk * 16 + (lane & 7) + ((mi >> 1) << 3);
+    const int chunk = 2 * warp + (mi & 1);
+    br::ldsm_x4_t(a, blk + tok * 128 + ((chunk ^ (lane & 7)) << 4));
+    // lane L draws group (token tok0 + (L & 15), features 8 ((feat0 >> 3) + (L >> 4)) ..)
+    xbuf[lane] = br::drop_group(d, tok0 + (lane & 15), (feat0 >> 3) + (lane >> 4), d.proj);
+    __syncwarp();
+    const uint16_t* b16 = reinterpret_cast<const uint16_t*>(xbuf);
+    const int fe = (lane >> 2) & 7, q = lane & 3;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int g = 8 * (i >> 1) + 2 * q + 16 * (i & 1);
+        a[i] &= br::keep_bits((uint32_t)b16[g * 8 + fe] | ((uint32_t)b16[(g + 1) * 8 + fe] << 16), d.T);   // tokens 2q | 2q + 1
+    }
+    __syncwarp();
+}
+
+template <int NPAD, bool MASK>
 __global__ void __launch_bounds__(NTHREADS, 1)
 tn_gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TnParams p) {
     constexpr int NBB = NPAD / 64;
@@ -85,8 +110,19 @@ tn_gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             for (int kk = 0; kk < BKT / 16; ++kk) {
                 // 16 tokens = 2 groups of 8 rows (SBO 1024 B); 64-wide feature / column blocks are 8192 B apart (LBO)
                 const uint64_t bd = br::wg_desc_mn(sa + A_BYTES + kk * 2048, B_BLK, 1024);
-                br::wgmma_ss<NPAD, 1, 1>(acc0, br::wg_desc_mn(sa + kk * 2048, 64 * 128, 1024), bd, 1);
-                br::wgmma_ss<NPAD, 1, 1>(acc1, br::wg_desc_mn(sa + 64 * 128 + kk * 2048, 64 * 128, 1024), bd, 1);
+                if constexpr (MASK) {
+                    uint4* xbuf = reinterpret_cast<uint4*>(smem + NSTAGE * STAGE + 256) + 32 * warp;
+                    const long long tok0 = p.drop.row0 + (long long)(kb_lo + i) * BKT + kk * 16;
+                    uint32_t a0[4], a1[4];
+                    masked_big_frag(a0, sa, kk, tok0, tile * BM + 16 * warp, p.drop, xbuf);
+                    masked_big_frag(a1, sa + 64 * 128, kk, tok0, tile * BM + 64 + 16 * warp, p.drop, xbuf);
+                    br::wg_fence();
+                    br::wgmma_rs<NPAD, 1>(acc0, a0, bd, 1);
+                    br::wgmma_rs<NPAD, 1>(acc1, a1, bd, 1);
+                } else {
+                    br::wgmma_ss<NPAD, 1, 1>(acc0, br::wg_desc_mn(sa + kk * 2048, 64 * 128, 1024), bd, 1);
+                    br::wgmma_ss<NPAD, 1, 1>(acc1, br::wg_desc_mn(sa + 64 * 128 + kk * 2048, 64 * 128, 1024), bd, 1);
+                }
             }
             br::wg_commit();
             br::wg_wait<0>();
@@ -95,6 +131,10 @@ tn_gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         }
         br::wg_fence_operand(acc0);
         br::wg_fence_operand(acc1);
+        if constexpr (MASK) {
+#pragma unroll
+            for (int c = 0; c < NPAD / 2; ++c) { acc0[c] *= p.drop.inv_keep; acc1[c] *= p.drop.inv_keep; }
+        }
         // every stage has been consumed and no load is in flight: the ring becomes the transpose buffer (one product row per thread)
         float* s_t = reinterpret_cast<float*>(smem);
         const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);
@@ -166,12 +206,12 @@ tn_gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     }
 }
 
-template <int NPAD>
+template <int NPAD, bool MASK = false>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, const TnParams& p, cudaStream_t st) {
     constexpr int NBB = NPAD / 64;
-    constexpr int SMEM = NSTAGE * (A_BYTES + NBB * B_BLK) + 256 + 1024;
+    constexpr int SMEM = NSTAGE * (A_BYTES + NBB * B_BLK) + 256 + (MASK ? 4 * 32 * 16 : 0) + 1024;   // + the masked draw exchange
     static_assert(NSTAGE * (A_BYTES + NBB * B_BLK) >= BM * (NPAD + 1) * 4, "transpose buffer");
-    auto kern = tn_gemm_tc5_kernel<NPAD>;
+    auto kern = tn_gemm_tc5_kernel<NPAD, MASK>;
     static bool done = false;
     if (!done) { BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM)); done = true; }
     kern<<<p.tiles * p.splits, NTHREADS, SMEM, st>>>(ta, tb, p);
@@ -188,8 +228,8 @@ int64_t br_lora_grad_workspace_bytes(void) {
     return (int64_t)br_num_sms() * 128 * BM * sizeof(float) + 4096 * sizeof(int);
 }
 
-int br_lora_grad_tn(const void* big, int64_t ldb, const void* small, int64_t lds, int M, int P, int N, int mode,
-                    const br_lora_grad_seg* segs, int n_seg, void* workspace, void* stream) {
+static int lora_grad_tn(const void* big, int64_t ldb, const void* small, int64_t lds, int M, int P, int N, int mode,
+                        const br_lora_grad_seg* segs, int n_seg, const br_lora_dropout* d, void* workspace, void* stream) {
     BR_CHECK_ARG(M > 0 && P > 0 && N >= 8 && N <= 128 && N % 8 == 0, "lora_grad_tn: M=%d P=%d N=%d (N %% 8, <= 128)", M, P, N);
     BR_CHECK_ARG(P % 8 == 0 && ldb % 8 == 0 && lds % 8 == 0 && ((uintptr_t)big % 16 == 0) && ((uintptr_t)small % 16 == 0), "lora_grad_tn: alignment");
     BR_CHECK_ARG(mode >= 0 && mode <= 2 && n_seg >= 1 && n_seg <= 3 && segs && workspace, "lora_grad_tn: bad mode / segments");
@@ -219,7 +259,23 @@ int br_lora_grad_tn(const void* big, int64_t ldb, const void* small, int64_t lds
     if ((rc = br_make_tmap_2d_bf16(&ta, big, (uint64_t)M, (uint64_t)P, (uint64_t)ldb, BKT))) return rc;
     if ((rc = br_make_tmap_2d_bf16(&tb, small, (uint64_t)M, (uint64_t)N, (uint64_t)lds, BKT))) return rc;
     cudaStream_t st = (cudaStream_t)stream;
+    if (d) {
+        p.drop = br::drop_params(*d);
+        return p.Npad == 64 ? launch<64, true>(ta, tb, p, st) : launch<128, true>(ta, tb, p, st);
+    }
     return p.Npad == 64 ? launch<64>(ta, tb, p, st) : launch<128>(ta, tb, p, st);
+}
+
+int br_lora_grad_tn(const void* big, int64_t ldb, const void* small, int64_t lds, int M, int P, int N, int mode,
+                    const br_lora_grad_seg* segs, int n_seg, void* workspace, void* stream) {
+    return lora_grad_tn(big, ldb, small, lds, M, P, N, mode, segs, n_seg, nullptr, workspace, stream);
+}
+
+int br_lora_grad_tn_dropout(const void* big, int64_t ldb, const void* small, int64_t lds, int M, int P, int N, int mode,
+                            const br_lora_grad_seg* segs, int n_seg, const br_lora_dropout* d, void* workspace, void* stream) {
+    int rc;
+    if ((rc = br::check_drop(d, "lora_grad_tn_dropout"))) return rc;
+    return lora_grad_tn(big, ldb, small, lds, M, P, N, mode, segs, n_seg, d, workspace, stream);
 }
 
 }  // extern "C"

@@ -67,7 +67,21 @@ template <int TA, int TB> struct WgSS<128, TA, TB> {      // D[64 x 128] (+)= A[
                      : BR_WG_F64(0) : "l"(a), "l"(b), "r"(accumulate), "n"(TA), "n"(TB));
     }
 };
-template <int TB> struct WgRS<64, TB> {                 // D[64 x 64] (+)= A[64 x 16] (registers) . B[16 x 64] (shared memory)
+template <int TB> struct WgRS<16, TB> {                 // D[64 x 16] (+)= A[64 x 16] (registers) . B[16 x 16] (shared memory)
+    static __device__ __forceinline__ void run(float (&d)[8], const uint32_t (&a)[4], uint64_t b, int accumulate) {
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"
+                     "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, %14;\n}\n"
+                     : BR_WG_F8(0) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(accumulate), "n"(TB));
+    }
+};
+template <int TB> struct WgRS<32, TB> {                 // D[64 x 32] (+)= A[64 x 16] (registers) . B[16 x 32] (shared memory)
+    static __device__ __forceinline__ void run(float (&d)[16], const uint32_t (&a)[4], uint64_t b, int accumulate) {
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+                     "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, %22;\n}\n"
+                     : BR_WG_F16(0) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(accumulate), "n"(TB));
+    }
+};
+template <int TB> struct WgRS<64, TB> {                // D[64 x 64] (+)= A[64 x 16] (registers) . B[16 x 64] (shared memory)
     static __device__ __forceinline__ void run(float (&d)[32], const uint32_t (&a)[4], uint64_t b, int accumulate) {
         asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
                      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n}\n"

@@ -64,6 +64,15 @@ class LoraW:
 
 
 @dataclass
+class LoraDropout:
+    """Dropout of one pass through the adapters (the mask rule is next to br_lora_dropout in include/bioreason_b200.h)."""
+    seed: int
+    pass_id: int             # advanced once per dropout-applying pass; every row chunk of a pass shares it
+    threshold: int           # T = round(p * 65536); p_eff = T / 65536
+    row_offset: int = 0      # global token row (b * L + t of the whole pass) of this chunk's first row
+
+
+@dataclass
 class LayerSaved:
     """Activations one decoder layer keeps for the hand-written backward."""
     h_in: torch.Tensor = None
@@ -98,20 +107,23 @@ def _rope_table(n_pos: int, D: int, theta: float, device):
     return t
 
 
-def _lin(x, w, *, lora_a=None, lora_b=None, lora_scale=1.0, saved_t=None, **kw):
-    """y = x @ w.T (+ (scale * x @ A.T) @ B.T as a second K segment of the same wgmma accumulation)."""
+def _lin(x, w, *, lora_a=None, lora_b=None, lora_scale=1.0, saved_t=None, drop=None, **kw):
+    """y = x @ w.T (+ (scale * x @ A.T) @ B.T as a second K segment of the same wgmma accumulation).
+    drop: optional br_lora_dropout of this linear's projections: t = scale / (1 - p_eff) * (x * m_j) @ A_j.T; the base GEMM reads x."""
     if lora_a is None:
         return ops.gemm(x, w, **kw), None
-    t = ops.gemm(x, lora_a, alpha=lora_scale)
+    t = ops.gemm(x, lora_a, alpha=lora_scale) if drop is None else ops.lora_down_dropout(x, lora_a, lora_scale, drop)
     return ops.gemm(x, w, a2=t, b2=lora_b, **kw), t
 
 
 def decoder_forward(W: DecoderW, h: torch.Tensor, B: int, L: int, positions: torch.Tensor, kv_start, kv_end, *,
                     lora: Optional[LoraW] = None, saved: Optional[List[LayerSaved]] = None,
-                    kv_sink: Optional[Callable[[int, torch.Tensor], None]] = None, final_norm: bool = True) -> torch.Tensor:
+                    kv_sink: Optional[Callable[[int, torch.Tensor], None]] = None, final_norm: bool = True,
+                    dropout: Optional[LoraDropout] = None) -> torch.Tensor:
     """Qwen3 decoder stack over dense rows [B, L] (HF qwen3/modeling_qwen3.py:294-336, 378-430).
 
     h: merged input embeddings [B*L, d] bf16 (not modified).  Returns the final-normed hidden states [B*L, d].
+    dropout: LoRA dropout of this pass (only with `lora`); None runs the adapters undropped.
     """
     cfg = W.cfg
     Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
@@ -123,13 +135,14 @@ def decoder_forward(W: DecoderW, h: torch.Tensor, B: int, L: int, positions: tor
     for li, Lw in enumerate(W.layers):
         lw = lora.layers[li] if lora is not None else None
         ls = lora.scale if lora is not None else 1.0
+        dd = (lambda j: ops.lora_dropout_desc(dropout, li, j, lora.r)) if (dropout is not None and lw is not None) else (lambda j: None)
         S = LayerSaved() if saved is not None else None
         if S is not None:
             xn, rstd1 = ops.rmsnorm(h, Lw.ln1, eps, want_rstd=True)
             S.h_in, S.rstd1, S.xn1 = h, rstd1, xn
         else:
             xn = ops.rmsnorm(h, Lw.ln1, eps)
-        qkv, t = _lin(xn, Lw.w_qkv, lora_a=lw.a_qkv if lw else None, lora_b=lw.b_qkv if lw else None, lora_scale=ls)
+        qkv, t = _lin(xn, Lw.w_qkv, lora_a=lw.a_qkv if lw else None, lora_b=lw.b_qkv if lw else None, lora_scale=ls, drop=dd(0))
         if S is not None:
             # training: the roped q|k go to their own buffer, the GEMM output keeps the pre-norm q|k (qk-norm backward) and V -- no copy
             S.t_qkv = t
@@ -148,7 +161,7 @@ def decoder_forward(W: DecoderW, h: torch.Tensor, B: int, L: int, positions: tor
             S.attn, S.lse = attn, lse
         else:
             attn = ops.attn_fwd(q, k, v, B, L, Hq, Hkv, D, kv_start=kv_start, kv_end=kv_end, causal=True)
-        h2, t = _lin(attn, Lw.w_o, lora_a=lw.a_o if lw else None, lora_b=lw.b_o if lw else None, lora_scale=ls, residual=h)
+        h2, t = _lin(attn, Lw.w_o, lora_a=lw.a_o if lw else None, lora_b=lw.b_o if lw else None, lora_scale=ls, residual=h, drop=dd(3))
         if S is not None:
             S.t_o = t
             xn2, rstd2 = ops.rmsnorm(h2, Lw.ln2, eps, want_rstd=True)
@@ -157,10 +170,10 @@ def decoder_forward(W: DecoderW, h: torch.Tensor, B: int, L: int, positions: tor
         else:
             xn2 = ops.rmsnorm(h2, Lw.ln2, eps)
             gu = None
-        act, t = _lin(xn2, Lw.w_gu, lora_a=lw.a_gu if lw else None, lora_b=lw.b_gu if lw else None, lora_scale=ls, act=1, aux_out=gu)
+        act, t = _lin(xn2, Lw.w_gu, lora_a=lw.a_gu if lw else None, lora_b=lw.b_gu if lw else None, lora_scale=ls, act=1, aux_out=gu, drop=dd(4))
         if S is not None:
             S.t_gu, S.gu, S.act = t, gu, act
-        h, t = _lin(act, Lw.w_down, lora_a=lw.a_down if lw else None, lora_b=lw.b_down if lw else None, lora_scale=ls, residual=h2)
+        h, t = _lin(act, Lw.w_down, lora_a=lw.a_down if lw else None, lora_b=lw.b_down if lw else None, lora_scale=ls, residual=h2, drop=dd(6))
         if S is not None:
             S.t_down = t
             saved.append(S)

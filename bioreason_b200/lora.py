@@ -5,8 +5,15 @@ every nn.Linear leaf of the text model except `lm_head` gets rank-r adapters (r=
 A ~ N(0, 1/r), B = 0), base weights frozen.  Module / parameter names follow peft (`base_layer`,
 `lora_A.default.weight`, `lora_B.default.weight`) so checkpoints keep their keys.  The fp32 master parameters are
 what the optimizer sees; `LoraState.sync()` re-packs them (bf16, fused/blocked like the base weights, plus the
-transposes the backward GEMMs read) after every optimizer step.  LoRA dropout is not applied (p = 0); the
-reference's 0.05 is a regulariser, not part of the path's arithmetic contract.
+transposes the backward GEMMs read) after every optimizer step.
+
+LoRA dropout is opt-in (`DNALLMModel.set_lora_dropout(p, seed)`; default p = 0, the undropped path).  When on, the training passes
+compute peft's y = base(x) + s * B(A(dropout(x))) with one counter-based mask per projection, regenerated in the backward instead
+of stored (rule next to br_lora_dropout in include/bioreason_b200.h).  It applies to the passes that train: the loss pass, the
+old-log-prob pass when num_iterations > 1, the SFT step with backward and the autograd bridge.  It never applies to the
+reference policy, to forward / per_token_logps, or to the rollout: the rollout samples from the merged, dropout-free policy
+(W + s B A), whereas the reference trainer stays in train mode through generate and samples through the dropped adapters.
+Dropout in decode would need unmerged adapters in the weight-streaming loop.
 """
 from __future__ import annotations
 
@@ -17,7 +24,7 @@ from typing import Dict, List
 import torch
 import torch.nn as nn
 
-from .engine import LoraLayerW, LoraW
+from .engine import LoraDropout, LoraLayerW, LoraW
 from .packing import gu_views
 
 TARGETS = ("q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj")
@@ -90,6 +97,30 @@ class LoraState:
             off += p.numel()
         self._alloc_packed(dec_w, dev)
         self.sync()
+        self.dropout = None                # (p, threshold T, seed) while LoRA dropout is on
+        self.dropout_pass = 0              # pass counter c of the masks: advanced once per dropout-applying pass
+
+    # ------------------------------------------------------------------
+    def set_dropout(self, p: float, seed: int = 0):
+        """p = 0 turns dropout off; 0 < p < 1 turns it on with T = round(p * 65536) (p_eff = T / 65536)."""
+        p = float(p)
+        if not 0.0 <= p < 1.0:
+            raise ValueError(f"LoRA dropout must lie in [0, 1), got {p}")
+        T = int(round(p * 65536))
+        if T >= 65536:
+            raise ValueError(f"LoRA dropout {p} rounds to p_eff = 1 at 16-bit resolution")
+        if T > 0 and self.r not in (16, 32, 64):
+            raise NotImplementedError(f"the LoRA dropout kernels are built for ranks 16, 32 and 64 (r = {self.r})")
+        self.dropout = (p, T, int(seed)) if T > 0 else None
+
+    def new_dropout_pass(self) -> int:
+        pid = self.dropout_pass
+        self.dropout_pass = (self.dropout_pass + 1) & 0xFFFFFFFF
+        return pid
+
+    def dropout_for(self, pass_id: int, row_offset: int) -> LoraDropout:
+        _, T, seed = self.dropout
+        return LoraDropout(seed=seed, pass_id=pass_id, threshold=T, row_offset=row_offset)
 
     # ------------------------------------------------------------------
     def _alloc_packed(self, W, dev):

@@ -228,6 +228,19 @@ class DNALLMModel(nn.Module):
         self._dec.build_transposes()
         return self._lora
 
+    def set_lora_dropout(self, p: float, seed: int = 0):
+        """peft's lora_dropout for the training passes (reason.py:376-384): p = 0 (the default) turns it off, 0 < p < 1 turns it on
+        with per-rank masks drawn from `seed`.  Needs the adapters (enable_lora / get_peft_model) first."""
+        if self._lora is None:
+            raise RuntimeError("set_lora_dropout needs LoRA adapters: call enable_lora first")
+        self._lora.set_dropout(p, seed)
+
+    def new_lora_dropout_pass(self) -> Optional[int]:
+        """Pass id shared by the row chunks of one dropout-applying pass (None while dropout is off)."""
+        if self._lora is None or self._lora.dropout is None:
+            return None
+        return self._lora.new_dropout_pass()
+
     @torch.no_grad()
     def merge_and_unload_lora(self):
         """peft's `merge_and_unload()` (reason.py:443-446): W <- W + (alpha/r) B A for every adapted projection, then drop the adapters

@@ -90,10 +90,24 @@ def _row_major_2d(t):
     return t.stride(0)
 
 
+def lora_dropout_desc(drop, layer: int, proj: int, r: int):
+    """br_lora_dropout for projection `proj` (lora.TARGETS index; block i of a fused linear is proj + i) of decoder layer `layer`.
+    drop: engine.LoraDropout (seed, pass id, threshold, row offset)."""
+    d = ffi.new("br_lora_dropout*")
+    d.seed = int(drop.seed) & 0xFFFFFFFFFFFFFFFF
+    setattr(d, "pass", int(drop.pass_id) & 0xFFFFFFFF)
+    d.layer, d.proj, d.r = int(layer), int(proj), int(r)
+    d.threshold = int(drop.threshold)
+    d.inv_keep = 65536.0 / (65536 - int(drop.threshold))
+    d.row_offset = int(drop.row_offset)
+    return d
+
+
 def gemm(a: torch.Tensor, b: torch.Tensor, *, bias=None, residual=None, alpha: float = 1.0, act: int = 0,
          out: Optional[torch.Tensor] = None, out_dtype=torch.bfloat16, row_map=None, aux_out=None,
-         a2=None, b2=None) -> torch.Tensor:
-    """out[M,N] = epilogue(a[M,K] @ b[N,K].T (+ a2[M,K2] @ b2[N,K2].T)) on wgmma (bf16 in, fp32 accumulate)."""
+         a2=None, b2=None, dropout=None) -> torch.Tensor:
+    """out[M,N] = epilogue(a[M,K] @ b[N,K].T (+ a2[M,K2] @ b2[N,K2].T)) on wgmma (bf16 in, fp32 accumulate).
+    dropout: optional br_lora_dropout (lora_dropout_desc): the a2 @ b2.T segment is a LoRA up-path whose r-wide K blocks are masked."""
     _need_cuda(a, b)
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16
     M, K = a.shape
@@ -121,6 +135,9 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, bias=None, residual=None, alpha: f
         assert a2.dtype == torch.bfloat16 and b2.dtype == torch.bfloat16 and a2.shape[0] == M and b2.shape[0] == N
         e.A2 = ptr(a2); e.lda2 = _row_major_2d(a2); e.B2 = ptr(b2); e.ldb2 = _row_major_2d(b2); e.K2 = a2.shape[1]
         keep += [a2, b2]
+    if dropout is not None:
+        assert a2 is not None, "the dropout mask applies to the second (LoRA) segment"
+        e.lora_dropout = dropout
     check(lib().br_gemm_bf16(ptr(a), _row_major_2d(a), ptr(b), _row_major_2d(b), ptr(out), _row_major_2d(out),
                              M, N, K, e, _stream()), "gemm_bf16")
     return out
@@ -359,10 +376,12 @@ def qk_rope_bwd_(dqkv, qk_pre, n_q, n_k, head_dim, q_norm_w, k_norm_w, positions
 _LORA_WS = {}
 
 
-def lora_grad_tn(big, small, segs, *, mode=0):
+def lora_grad_tn(big, small, segs, *, mode=0, dropout=None):
     """Deterministic wgmma TN GEMM: product[P, N] = big[M, P]^T @ small[M, N]; the blocks named by `segs` are ADDED into fp32 views.
     segs: list of (dst fp32 2-D view with contiguous rows, row_lo, row_hi, col_lo, n_cols); mode 1: one segment, dst[n, p] (transposed);
-    mode 2: gate/up-blocked product rows (segment 0 = gate rows, 1 = up rows)."""
+    mode 2: gate/up-blocked product rows (segment 0 = gate rows, 1 = up rows).
+    dropout: optional br_lora_dropout (lora_dropout_desc): `big` is the adapter input x, masked, and the product is scaled by
+    1 / (1 - p_eff), i.e. dA += inv_keep * u^T (x * m)."""
     _need_cuda(big, small)
     assert big.dtype == torch.bfloat16 and small.dtype == torch.bfloat16 and big.shape[0] == small.shape[0]
     M, P = big.shape
@@ -376,8 +395,33 @@ def lora_grad_tn(big, small, segs, *, mode=0):
         assert dst.dtype == torch.float32 and dst.dim() == 2 and dst.stride(1) == 1
         arr[i].dst = ptr(dst, "float*"); arr[i].ld = dst.stride(0)
         arr[i].row_lo, arr[i].row_hi, arr[i].col_lo, arr[i].n_cols = int(row_lo), int(row_hi), int(col_lo), int(n_cols)
+    if dropout is not None:
+        check(lib().br_lora_grad_tn_dropout(ptr(big), _row_major_2d(big), ptr(small), _row_major_2d(small), M, P, N, int(mode), arr, len(segs),
+                                            dropout, ptr(ws), _stream()), "lora_grad_tn_dropout")
+        return
     check(lib().br_lora_grad_tn(ptr(big), _row_major_2d(big), ptr(small), _row_major_2d(small), M, P, N, int(mode), arr, len(segs), ptr(ws),
                                 _stream()), "lora_grad_tn")
+
+
+def lora_down_dropout(x, a, scale: float, dropout, out=None):
+    """t[M, n_proj * r] = scale / (1 - p_eff) * ((x * m_j) @ A_j.T) for the stacked adapters a [n_proj * r, K] of one fused linear."""
+    _need_cuda(x, a)
+    assert x.dtype == torch.bfloat16 and a.dtype == torch.bfloat16
+    M, K = x.shape
+    n_proj = a.shape[0] // dropout.r
+    assert a.shape[0] == n_proj * dropout.r and a.shape[1] == K
+    if out is None:
+        out = torch.empty(M, a.shape[0], device=x.device, dtype=torch.bfloat16)
+    check(lib().br_lora_down_dropout(ptr(x), _row_major_2d(x), ptr(a), _row_major_2d(a), ptr(out), _row_major_2d(out), M, K, n_proj,
+                                     float(scale), dropout, _stream()), "lora_down_dropout")
+    return out
+
+
+def lora_dropout_mask(dropout, M: int, K: int, device) -> torch.Tensor:
+    """uint8 [M, K]: 1 where element (row_offset + m, k) of projection dropout.proj's input is kept."""
+    keep = torch.empty(M, K, device=device, dtype=torch.uint8)
+    check(lib().br_lora_dropout_mask(dropout, M, K, ffi.cast("uint8_t*", keep.data_ptr()), K, _stream()), "lora_dropout_mask")
+    return keep
 
 
 def transpose(x, out=None, pad_cols_to: int = 8):

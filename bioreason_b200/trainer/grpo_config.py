@@ -65,7 +65,8 @@ class DNALLMGRPOConfig:
     eval_strategy: str = "no"
     save_steps: int = 0                   # > 0: fire the callbacks' on_save every save_steps optimizer steps (HF save_strategy="steps")
     save_safetensors: bool = False        # reason.py:597 sets it; saving itself is the callbacks' job (reason.py:46-81)
-    lora_dropout: float = 0.05            # accepted; the kernels apply no dropout (DESIGN.md: out of scope)
+    lora_dropout: float = 0.05            # the rate apply_lora_dropout uses when compat.peft recorded none
+    apply_lora_dropout: bool = False      # train through LoRA dropout (off: the undropped path, bit-identical to before)
     # additions of this implementation
     lora_r: int = 32
     lora_alpha: float = 64.0

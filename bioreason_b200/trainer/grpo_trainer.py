@@ -113,6 +113,9 @@ class DNALLMGRPOTrainer:
         if model._lora is None:
             model.enable_lora(r=a.lora_r, alpha=a.lora_alpha, seed=a.seed)
         model.sync_adapters(rollout=True)
+        if a.apply_lora_dropout:                                            # peft's rate; per-rank masks (set_seed(device_specific=True))
+            p = getattr(model, "lora_dropout", None)
+            model.set_lora_dropout(a.lora_dropout if p is None else p, seed=a.seed + rank)
         self.eos_token_id = getattr(processing_class, "eos_token_id", None) if processing_class is not None else None
         if self.eos_token_id is None:
             self.eos_token_id = model.text_config.eos_token_id
@@ -200,12 +203,12 @@ class DNALLMGRPOTrainer:
         return out
 
     # ------------------------------------------------------------------ log-probs
-    def _get_per_token_logps(self, model, input_ids, attention_mask, keep_last=None, lora="policy", **mm):
+    def _get_per_token_logps(self, model, input_ids, attention_mask, keep_last=None, lora="policy", dropout=False, **mm):
         """grpo_trainer.py:510-520 (+ the [:, P-1:] slice of :779 when keep_last is given), no-grad version."""
         n = input_ids.shape[1] - 1 if keep_last is None else keep_last
         with torch.no_grad():
             lp, _ = training.policy_forward(model, input_ids, attention_mask, mm.get("dna_tokenized"), mm.get("batch_idx_map"), n,
-                                            save=False, lora=lora)
+                                            save=False, lora=lora, dropout=dropout)
         return lp
 
     # ------------------------------------------------------------------ rollout + scoring
@@ -236,7 +239,8 @@ class DNALLMGRPOTrainer:
         attention_mask = torch.cat([prompt_mask, completion_mask.to(prompt_mask.dtype)], dim=1)                       # :612
         Cc = completion_ids.shape[1]
         with self._mark("ref_logps"):
-            old_lp = self._get_per_token_logps(model, ids, attention_mask, keep_last=Cc, **mm) if self.num_iterations > 1 else None
+            # the reference computes old log-probs in train mode: through the LoRA dropout when it is on
+            old_lp = self._get_per_token_logps(model, ids, attention_mask, keep_last=Cc, dropout=True, **mm) if self.num_iterations > 1 else None
             ref_lp = self._get_per_token_logps(model, ids, attention_mask, keep_last=Cc, lora=None, **mm) if self.beta != 0.0 else None
         # rewards: the reference protocol f(prompts=, completions=, **columns) on decoded text (:640-676); functions that name a
         # `completion_ids` parameter get device tensors instead (trainer/rewards.py)
@@ -290,13 +294,17 @@ class DNALLMGRPOTrainer:
         mr = self.args.micro_rows or (self._auto_micro_rows(model, B, ids.shape[1]) if ids.is_cuda else B)
         ga = self.args.gradient_accumulation_steps
         loss_acc = torch.zeros(3, device=ids.device)
+        # one LoRA-dropout pass for all row chunks; each chunk passes its first row so the masks ignore the chunking
+        pid = model.new_lora_dropout_pass() if getattr(model, "_lora", None) is not None else None
         for lo in range(0, B, mr):
             hi = min(B, lo + mr)
             sl = slice(lo, hi)
             mm_c = _slice_mm(mm, lo, hi)
             t0 = time.perf_counter()
             with self._mark("policy_fwd"):
-                lp, ctx = training.policy_forward(model, ids[sl], mask[sl], mm_c["dna_tokenized"], mm_c["batch_idx_map"], C, save=backward)
+                drop_kw = dict(dropout=True, dropout_pass=pid, row_offset=lo) if pid is not None else {}
+                lp, ctx = training.policy_forward(model, ids[sl], mask[sl], mm_c["dna_tokenized"], mm_c["batch_idx_map"], C, save=backward,
+                                                  **drop_kw)
             out3, dlp = ops.grpo_loss_raw(lp, old[sl] if old is not None else None, ref[sl] if ref is not None else None, adv[sl],
                                           completion_mask[sl], self.beta, self.epsilon_low, self.epsilon_high, want_grad=backward)
             w = (hi - lo) / B

@@ -13,6 +13,7 @@ import torch
 
 from . import engine, ops
 from .engine import LayerSaved
+from .lora import TARGETS
 
 
 class PolicyCtx:
@@ -33,10 +34,14 @@ def activation_bytes_per_token(model) -> int:
 
 
 def policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_map, keep_last: int, *, save: bool = True,
-                   lora="policy", targets: Optional[torch.Tensor] = None) -> "tuple[torch.Tensor, Optional[PolicyCtx]]":
+                   lora="policy", targets: Optional[torch.Tensor] = None, dropout: bool = False, dropout_pass: Optional[int] = None,
+                   row_offset: int = 0) -> "tuple[torch.Tensor, Optional[PolicyCtx]]":
     """Returns (logps [B, keep_last] fp32, ctx).  lora: "policy" (adapters on), None (base weights = reference policy).
     targets: optional [B, keep_last] class ids scored at the last keep_last positions before the end (default: the realised next
-    tokens input_ids[:, L-keep_last:]); entries < 0 are ignored (log-prob 0, no gradient) -- the SFT label mask."""
+    tokens input_ids[:, L-keep_last:]); entries < 0 are ignored (log-prob 0, no gradient) -- the SFT label mask.
+    dropout: apply the LoRA dropout set by `model.set_lora_dropout` (no-op while it is off or with lora=None).  Row chunks of one pass
+    share `dropout_pass` (from `model.new_lora_dropout_pass()`; None draws a new pass) and give `row_offset` = the batch row of their
+    first row, so the masks do not depend on the chunking.  policy_backward regenerates the same masks from ctx."""
     W = model._dec
     dev = W.embed.device
     input_ids = input_ids.to(dev)
@@ -56,7 +61,11 @@ def policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_ma
     ks, ke = engine.mask_window(attention_mask)
     pos = engine.forward_positions(B, L, dev)
     saved: Optional[List[LayerSaved]] = [] if save else None
-    h = engine.decoder_forward(W, emb, B, L, pos, ks, ke, lora=use_lora, saved=saved, final_norm=False)
+    drop = None
+    if dropout and use_lora is not None and model._lora.dropout is not None:
+        pid = model._lora.new_dropout_pass() if dropout_pass is None else dropout_pass
+        drop = model._lora.dropout_for(pid, row_offset * L)
+    h = engine.decoder_forward(W, emb, B, L, pos, ks, ke, lora=use_lora, saved=saved, final_norm=False, dropout=drop)
     eps = W.cfg.rms_norm_eps
     if save:
         hn, rstd_f = ops.rmsnorm(h, W.final_norm, eps, want_rstd=True)
@@ -76,6 +85,7 @@ def policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_ma
         ctx.rows, ctx.h_sel, ctx.tgt, ctx.lse = rows, h_sel, tgt, lse
         ctx.pos, ctx.ks, ctx.ke, ctx.aux = pos, ks, ke, aux
         ctx.use_lora = use_lora is not None
+        ctx.drop = drop
     return logp.view(B, n), ctx
 
 
@@ -108,12 +118,19 @@ def policy_backward(model, ctx: PolicyCtx, dlogp: torch.Tensor, on_layer_done=No
     dh = ops.rmsnorm_bwd(ctx.h_final, W.final_norm, ctx.rstd_f, dhn)
     del dhn
 
+    drop = getattr(ctx, "drop", None)
+
+    def dd(li, j):
+        """mask descriptor of projection j (lora.TARGETS index) in layer li, or None without dropout"""
+        return ops.lora_dropout_desc(drop, li, j, r) if drop is not None else None
+
     def lin_bwd(dy, w_T, x_in, t_saved, li, names, a_T, b_T, big_cols=None, **kw):
-        """dx = dy @ W (+ LoRA path) and LoRA grads.  names: LoRA target names fused in this linear (in packed order)."""
+        """dx = dy @ W (+ LoRA path) and LoRA grads.  names: LoRA target names fused in this linear (in packed order).
+        With dropout the u @ A segment is masked per projection: dx = dy @ W + sum_j m_j * inv_keep * (u_j @ A_j)."""
         if lora is None:
             return ops.gemm(dy, w_T, **kw)
         u = ops.gemm(dy, b_T, alpha=s)                                    # [M, r * len(names)] = s * dy @ B
-        dx = ops.gemm(dy, w_T, a2=u, b2=a_T, **kw)
+        dx = ops.gemm(dy, w_T, a2=u, b2=a_T, dropout=dd(li, TARGETS.index(names[0])), **kw)
         return dx, u
 
     for li in range(len(W.layers) - 1, -1, -1):
@@ -123,7 +140,7 @@ def policy_backward(model, ctx: PolicyCtx, dlogp: torch.Tensor, on_layer_done=No
         if lora:
             dact, u = lin_bwd(dh, Lw.w_down_T, S.act, S.t_down, li, ("down_proj",), Tl["a_down_T"], Tl["b_down_T"])
             ops.lora_grad_tn(dh, S.t_down, [(lora.grad_view(li, "down_proj", "B"), 0, d, 0, r)])               # dB = dy^T t
-            ops.lora_grad_tn(S.act, u, [(lora.grad_view(li, "down_proj", "A"), 0, F, 0, r)], mode=1)           # dA = u^T x
+            ops.lora_grad_tn(S.act, u, [(lora.grad_view(li, "down_proj", "A"), 0, F, 0, r)], mode=1, dropout=dd(li, 6))  # dA = u^T x
         else:
             dact = ops.gemm(dh, Lw.w_down_T)
         dgu = ops.swiglu_bwd(S.gu, dact)
@@ -133,8 +150,8 @@ def policy_backward(model, ctx: PolicyCtx, dlogp: torch.Tensor, on_layer_done=No
             # one product dgu^T [2F] x t_gu [2r]: gate rows keep their r columns, up rows theirs (cross blocks are discarded)
             ops.lora_grad_tn(dgu, S.t_gu, [(lora.grad_view(li, "gate_proj", "B"), 0, 2 * F, 0, r),
                                            (lora.grad_view(li, "up_proj", "B"), 0, 2 * F, r, r)], mode=2)
-            ops.lora_grad_tn(S.xn2, u[:, :r], [(lora.grad_view(li, "gate_proj", "A"), 0, d, 0, r)], mode=1)
-            ops.lora_grad_tn(S.xn2, u[:, r:], [(lora.grad_view(li, "up_proj", "A"), 0, d, 0, r)], mode=1)
+            ops.lora_grad_tn(S.xn2, u[:, :r], [(lora.grad_view(li, "gate_proj", "A"), 0, d, 0, r)], mode=1, dropout=dd(li, 4))
+            ops.lora_grad_tn(S.xn2, u[:, r:], [(lora.grad_view(li, "up_proj", "A"), 0, d, 0, r)], mode=1, dropout=dd(li, 5))
         else:
             dxn2 = ops.gemm(dgu, Lw.w_gu_T)
         del dgu
@@ -144,7 +161,7 @@ def policy_backward(model, ctx: PolicyCtx, dlogp: torch.Tensor, on_layer_done=No
         if lora:
             dattn, u = lin_bwd(dh_mid, Lw.w_o_T, S.attn, S.t_o, li, ("o_proj",), Tl["a_o_T"], Tl["b_o_T"])
             ops.lora_grad_tn(dh_mid, S.t_o, [(lora.grad_view(li, "o_proj", "B"), 0, d, 0, r)])
-            ops.lora_grad_tn(S.attn, u, [(lora.grad_view(li, "o_proj", "A"), 0, Hq * D, 0, r)], mode=1)
+            ops.lora_grad_tn(S.attn, u, [(lora.grad_view(li, "o_proj", "A"), 0, Hq * D, 0, r)], mode=1, dropout=dd(li, 3))
         else:
             dattn = ops.gemm(dh_mid, Lw.w_o_T)
         dqkv = torch.empty(M, (Hq + 2 * Hkv) * D, device=dev, dtype=torch.bfloat16)
@@ -158,7 +175,7 @@ def policy_backward(model, ctx: PolicyCtx, dlogp: torch.Tensor, on_layer_done=No
             ops.lora_grad_tn(dqkv, S.t_qkv, [(lora.grad_view(li, "q_proj", "B"), qo, ko, 0, r), (lora.grad_view(li, "k_proj", "B"), ko, vo, r, r),
                                              (lora.grad_view(li, "v_proj", "B"), vo, vo + Hkv * D, 2 * r, r)])
             for j, name in enumerate(("q_proj", "k_proj", "v_proj")):
-                ops.lora_grad_tn(S.xn1, u[:, j * r:(j + 1) * r], [(lora.grad_view(li, name, "A"), 0, d, 0, r)], mode=1)
+                ops.lora_grad_tn(S.xn1, u[:, j * r:(j + 1) * r], [(lora.grad_view(li, name, "A"), 0, d, 0, r)], mode=1, dropout=dd(li, j))
         else:
             dxn1 = ops.gemm(dqkv, Lw.w_qkv_T)
         del dqkv
@@ -182,14 +199,16 @@ def policy_backward(model, ctx: PolicyCtx, dlogp: torch.Tensor, on_layer_done=No
 
 def sft_step(model, input_ids, attention_mask, dna_tokenized, batch_idx_map, labels, *, backward: bool = True, grad_scale: float = 1.0):
     """One supervised step (train_dna_qwen.py:179-213 -> HF ForCausalLMLoss, loss/loss_utils.py:28-67): shift, ignore -100, mean CE.
-    Returns the loss; with backward=True accumulates d(loss * grad_scale) into the LoRA / projector gradient buffers."""
+    Returns the loss; with backward=True accumulates d(loss * grad_scale) into the LoRA / projector gradient buffers (through the LoRA
+    dropout when it is on; the forward-only loss is undropped, like eval mode)."""
     dev = model._dec.embed.device
     labels = labels.to(dev)
     B, L = labels.shape
     tgt = torch.where(labels[:, 1:] == -100, torch.full_like(labels[:, 1:], -1), labels[:, 1:])           # position t predicts label t+1
     valid = tgt >= 0
     n = valid.sum().clamp(min=1).float()
-    lp, ctx = policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_map, L - 1, save=backward, targets=tgt)
+    lp, ctx = policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_map, L - 1, save=backward, targets=tgt,
+                             dropout=backward)
     loss = -(lp * valid).sum() / n
     if backward:
         policy_backward(model, ctx, (-(valid.float()) / n) * grad_scale)
@@ -201,7 +220,7 @@ class _PolicyLogps(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model, input_ids, attention_mask, dna_tokenized, batch_idx_map, keep_last, *trainable):
-        logp, pctx = policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_map, keep_last, save=True)
+        logp, pctx = policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_map, keep_last, save=True, dropout=True)
         ctx.model, ctx.pctx, ctx.n_train = model, pctx, len(trainable)
         return logp
 

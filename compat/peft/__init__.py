@@ -66,7 +66,7 @@ def get_peft_model(model, peft_config: LoraConfig, adapter_name: str = "default"
         raise NotImplementedError("LoRA bias training is not on this path (the reference uses bias='none', reason.py:382)")
     if adapter_name != "default":
         raise NotImplementedError("one adapter named 'default'")
-    owner.lora_dropout = float(peft_config.lora_dropout)       # recorded; the kernels apply no dropout (DESIGN.md: out of scope)
+    owner.lora_dropout = float(peft_config.lora_dropout)       # recorded; the trainer applies it with DNALLMGRPOConfig.apply_lora_dropout
     owner.enable_lora(r=int(peft_config.r), alpha=float(peft_config.lora_alpha))
     return model
 

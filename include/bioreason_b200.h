@@ -50,6 +50,23 @@ int br_eos_mask(const int64_t* completion_ids, int B, int C, int64_t eos_id, int
  * Dense contractions on wgmma (replaces every nn.Linear / lm_head reached through
  * dna_llm.py:150-160,237-242; SURVEY.md §2.3 K1,K2,K5,K6,K7,K12)
  * ------------------------------------------------------------------------------------------- */
+/* LoRA dropout (peft: y = base(x) + s * B(A(dropout(x)))) with a counter-based mask that is never stored: element (row, col) of the
+ * input of projection j in decoder layer l, in pass c, is kept iff bits >= threshold, where
+ *   w    = Philox4x32-10(counter = (col >> 3, row, (l << 3) | j, c), key = (seed mod 2^32, seed >> 32))
+ *   bits = (w[(col & 7) >> 1] >> (16 * (col & 1))) & 0xFFFF
+ * and kept elements are scaled by inv_keep.  row is the global token row (row_offset + local row), so chunked calls reproduce the
+ * mask of the whole pass. */
+typedef struct br_lora_dropout {
+    uint64_t seed;
+    uint32_t pass;           /* c: advanced once per dropout-applying pass */
+    int32_t layer;           /* l */
+    int32_t proj;            /* j of the first r-wide block (q 0, k 1, v 2, o 3, gate 4, up 5, down 6); block i is projection proj + i */
+    int32_t r;               /* adapter rank: columns per projection (multiple of 16, <= 64) */
+    int32_t threshold;       /* T = round(p * 65536), 1..65535 */
+    float inv_keep;          /* 65536 / (65536 - T) */
+    int64_t row_offset;      /* global token row of local row 0 */
+} br_lora_dropout;
+
 typedef struct br_gemm_epilogue {
     const void* bias;        /* [N] or NULL */
     int32_t bias_dtype;      /* BR_BF16 / BR_F32 */
@@ -66,6 +83,9 @@ typedef struct br_gemm_epilogue {
     const void* B2;
     int64_t ldb2;
     int32_t K2;
+    const br_lora_dropout* lora_dropout;   /* optional (NULL: unmasked): the second segment is a LoRA up-path u . A; the product of
+                                            each r-wide K block (projection proj + i) is multiplied by that projection's mask over
+                                            [M, N] and by inv_keep before it joins the accumulator (dx of the dropped input) */
 } br_gemm_epilogue;
 
 /* D[M, N] = epilogue(A[M, K] . B[N, K]^T); A, B bf16 row-major (K contiguous); ld* in elements. */
@@ -199,6 +219,16 @@ typedef struct br_lora_grad_seg { float* dst; int64_t ld; int32_t row_lo, row_hi
 int64_t br_lora_grad_workspace_bytes(void);
 int br_lora_grad_tn(const void* big, int64_t ldb, const void* small, int64_t lds, int M, int P, int N, int mode,
                     const br_lora_grad_seg* segs, int n_seg, void* workspace, void* stream);
+/* Same product with the dropout mask of projection d->proj applied to `big` (features = mask columns, tokens = mask rows) and the
+ * result scaled by d->inv_keep: dA = inv_keep * u^T (x . m) for one adapter (mode 1). */
+int br_lora_grad_tn_dropout(const void* big, int64_t ldb, const void* small, int64_t lds, int M, int P, int N, int mode,
+                            const br_lora_grad_seg* segs, int n_seg, const br_lora_dropout* d, void* workspace, void* stream);
+/* LoRA down-projection with dropout (forward): t[M, n_proj * r] = scale * inv_keep * ((x . m_j) . A_j^T) for the n_proj stacked
+ * adapters A [n_proj * r, K] of one fused linear (j = d->proj + block), bf16 out; x is read once for all of them. */
+int br_lora_down_dropout(const void* x, int64_t ldx, const void* A, int64_t lda, void* t, int64_t ldt, int M, int K, int n_proj,
+                         float scale, const br_lora_dropout* d, void* stream);
+/* keep[m, k] = 1 if element (row_offset + m, k) of projection d->proj's input is kept, else 0 (uint8 [M, ldo]; tests / inspection) */
+int br_lora_dropout_mask(const br_lora_dropout* d, int M, int K, uint8_t* keep, int64_t ldo, void* stream);
 int br_transpose_bf16(const void* in, int64_t ldi, void* out, int64_t ldo, int M, int N, void* stream);
 int br_colsum_accumulate(const void* in, int64_t ldi, float* out, int M, int N, void* stream);
 
