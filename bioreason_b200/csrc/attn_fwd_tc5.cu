@@ -4,6 +4,11 @@
 // [kv_start[b], kv_end[b]) (one contiguous window: left pads / post-EOS tail are outside), j <= i when causal; optional
 // log-sum-exp output for the backward.
 //
+// Shared-prefix mode (SHARED = true, causal D = 128 only; br_attn_fwd_shared): the token buffer holds U groups of G rows as
+// [U * Lp prefix rows | R = U * G suffixes of Ls rows], Lp a multiple of 64.  A CTA handles a query tile of suffix row r; key tiles
+// j < Lp / 64 come from group r / G's prefix rows, later ones from row r's suffix.  Tiles, tile order and masks are those of the dense
+// kernel on the equivalent [R, Lp + Ls] row, so O and the log-sum-exp are bit-identical to it.
+//
 // One CTA = one warpgroup = one 64-query tile of one (batch row, query head); 80 KB of shared memory at D = 128 (two CTAs per SM),
 // 48 KB at D = 64 (four).  Thread 0 issues the TMA
 // loads: the Q tile once, K and V tiles (64 keys x D, 128B-swizzled 64-column boxes) through a two-stage ring, so tile t+1 lands
@@ -26,6 +31,9 @@ struct FwdParams {
     int B, L, Hq, Hkv;
     const int *kv_start, *kv_end;
     float scale_log2;            // softmax scale * log2(e)
+    // shared-prefix mode: L = Lp + Ls, B = R suffix rows, kv_start per group ([R / G]), kv_end per row, lse [R, Hq, Ls]
+    int G, Lp, Ls;
+    long long sfx0;              // first suffix row of the buffer (U * Lp)
 };
 
 __device__ __forceinline__ float ex2(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
@@ -42,7 +50,7 @@ struct SL {
     static constexpr int TOTAL = OFF_BAR + 64 + 1024;
 };
 
-template <int D, bool CAUSAL>
+template <int D, bool CAUSAL, bool SHARED>
 __global__ void __launch_bounds__(NTHREADS, 2)
 attn_fwd_tc5_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                     const FwdParams p) {
@@ -53,11 +61,11 @@ attn_fwd_tc5_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     uint64_t* kv_full = q_full + 1;                // 2
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int qb = gridDim.x - 1 - blockIdx.x;     // heavy (late) causal tiles first
+    const int qb = (SHARED ? p.Lp / BM : 0) + gridDim.x - 1 - blockIdx.x;     // heavy (late) causal tiles first
     const int h = blockIdx.y, b = blockIdx.z;
     const int hk = h / (p.Hq / p.Hkv);
     const int q0 = qb * BM;
-    const int ks = p.kv_start ? p.kv_start[b] : 0;
+    const int ks = p.kv_start ? p.kv_start[SHARED ? b / p.G : b] : 0;
     const int ke = p.kv_end ? p.kv_end[b] : p.L;
     int last_key = ke - 1;
     if (CAUSAL) last_key = min(last_key, q0 + BM - 1);
@@ -66,8 +74,11 @@ attn_fwd_tc5_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     if (ke <= ks) jb_hi = jb_lo - 1;
     const int n_tiles = max(0, jb_hi - jb_lo + 1);
 
+    // buffer row of position i of this CTA's row (queries and outputs: i >= Lp in shared mode)
+    auto tok_row = [&](int i) -> long long { return SHARED ? p.sfx0 + (long long)b * p.Ls + (i - p.Lp) : (long long)b * p.L + i; };
     auto load_kv = [&](int t) {
-        const int st = t & 1, row_k = b * p.L + (jb_lo + t) * BN;
+        const int st = t & 1, j0 = (jb_lo + t) * BN;
+        const int row_k = SHARED ? (j0 < p.Lp ? (b / p.G) * p.Lp + j0 : (int)tok_row(j0)) : b * p.L + j0;
         br::mbar_expect_tx(&kv_full[st], 2 * L::TILE);
 #pragma unroll
         for (int nb = 0; nb < L::NB; ++nb) {
@@ -82,7 +93,7 @@ attn_fwd_tc5_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         if (n_tiles > 0) {
             br::mbar_expect_tx(q_full, L::TILE);
 #pragma unroll
-            for (int nb = 0; nb < L::NB; ++nb) br::tma_load_2d(smem + L::OFF_Q + nb * L::BLK, &tmQ, q_full, h * D + nb * 64, b * p.L + q0);
+            for (int nb = 0; nb < L::NB; ++nb) br::tma_load_2d(smem + L::OFF_Q + nb * L::BLK, &tmQ, q_full, h * D + nb * 64, (int)tok_row(q0));
             load_kv(0);
             if (n_tiles > 1) load_kv(1);
         }
@@ -177,28 +188,29 @@ attn_fwd_tc5_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         const int i_glob = q0 + r0 + 8 * hh;
         if (i_glob >= p.L) continue;
         const float inv = lt > 0.f ? 1.f / lt : 0.f;
-        bf16* orow = p.o + ((long long)b * p.L + i_glob) * p.ldo + (long long)h * D;
+        bf16* orow = p.o + tok_row(i_glob) * p.ldo + (long long)h * D;
 #pragma unroll
         for (int i = 0; i < D / 8; ++i)
             *reinterpret_cast<uint32_t*>(orow + 8 * i + cq) = br::pack_bf16(o_acc[4 * i + 2 * hh] * inv, o_acc[4 * i + 2 * hh + 1] * inv);
         if (p.lse && (lane & 3) == 0) {
             const float LN2 = 0.6931471805599453f;
-            p.lse[((long long)b * p.Hq + h) * p.L + i_glob] = lt > 0.f ? m_used[hh] * LN2 + logf(lt) : INFINITY;
+            const long long li = SHARED ? ((long long)b * p.Hq + h) * p.Ls + i_glob - p.Lp : ((long long)b * p.Hq + h) * p.L + i_glob;
+            p.lse[li] = lt > 0.f ? m_used[hh] * LN2 + logf(lt) : INFINITY;
         }
     }
 }
 
-template <int D, bool CAUSAL>
+template <int D, bool CAUSAL, bool SHARED = false>
 int launch(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const FwdParams& p, cudaStream_t st) {
     using L = SL<D>;
-    auto kern = attn_fwd_tc5_kernel<D, CAUSAL>;
+    auto kern = attn_fwd_tc5_kernel<D, CAUSAL, SHARED>;
     static bool done = false;
     if (!done) {
         BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
         BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100));       // several CTAs per SM
         done = true;
     }
-    dim3 grid((p.L + BM - 1) / BM, p.Hq, p.B);
+    dim3 grid(((SHARED ? p.Ls : p.L) + BM - 1) / BM, p.Hq, p.B);
     kern<<<grid, NTHREADS, L::TOTAL, st>>>(tq, tk, tv, p);
     BR_CHECK_LAUNCH();
     return BR_OK;
@@ -209,7 +221,7 @@ int launch(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, 
 int br_attn_fwd_tc5_impl(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o, int64_t ldo, float* lse,
                          int B, int L, int n_q_heads, int n_kv_heads, int head_dim, const int32_t* kv_start, const int32_t* kv_end,
                          float scale, int causal, cudaStream_t st) {
-    FwdParams p;
+    FwdParams p = {};
     p.o = (bf16*)o; p.ldo = ldo; p.lse = lse; p.B = B; p.L = L; p.Hq = n_q_heads; p.Hkv = n_kv_heads;
     p.kv_start = kv_start; p.kv_end = kv_end; p.scale_log2 = scale * 1.4426950408889634f;
     BR_CHECK_ARG(((uintptr_t)q % 16 == 0) && ((uintptr_t)k % 16 == 0) && ((uintptr_t)v % 16 == 0) && ((uintptr_t)o % 16 == 0),
@@ -222,4 +234,26 @@ int br_attn_fwd_tc5_impl(const void* q, int64_t ldq, const void* k, int64_t ldk,
     if ((rc = br_make_tmap_2d_bf16(&tv, v, rows, (uint64_t)n_kv_heads * head_dim, ldv, BN))) return rc;
     if (head_dim == 128) return causal ? launch<128, true>(tq, tk, tv, p, st) : launch<128, false>(tq, tk, tv, p, st);
     return causal ? launch<64, true>(tq, tk, tv, p, st) : launch<64, false>(tq, tk, tv, p, st);
+}
+
+int br_attn_fwd_shared_tc5_impl(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o, int64_t ldo,
+                                float* lse_prefix, float* lse_suffix, int U, int G, int Lp, int Ls, int n_q_heads, int n_kv_heads,
+                                const int32_t* kv_start, const int32_t* kv_end, float scale, cudaStream_t st) {
+    BR_CHECK_ARG(((uintptr_t)q % 16 == 0) && ((uintptr_t)k % 16 == 0) && ((uintptr_t)v % 16 == 0) && ((uintptr_t)o % 16 == 0),
+                 "attn_fwd_shared: q/k/v/o must be 16-byte aligned");
+    const uint64_t rows = (uint64_t)U * Lp + (uint64_t)U * G * Ls;
+    CUtensorMap tq, tk, tv;
+    int rc;
+    if ((rc = br_make_tmap_2d_bf16(&tq, q, rows, (uint64_t)n_q_heads * 128, ldq, BM))) return rc;
+    if ((rc = br_make_tmap_2d_bf16(&tk, k, rows, (uint64_t)n_kv_heads * 128, ldk, BN))) return rc;
+    if ((rc = br_make_tmap_2d_bf16(&tv, v, rows, (uint64_t)n_kv_heads * 128, ldv, BN))) return rc;
+    FwdParams p = {};
+    p.o = (bf16*)o; p.ldo = ldo; p.Hq = n_q_heads; p.Hkv = n_kv_heads; p.kv_start = kv_start; p.scale_log2 = scale * 1.4426950408889634f;
+    if (Lp > 0) {                                   // prefix rows: the dense kernel on [U, Lp] (prefix queries see prefix keys only)
+        p.lse = lse_prefix; p.B = U; p.L = Lp; p.kv_end = nullptr;
+        if ((rc = launch<128, true>(tq, tk, tv, p, st))) return rc;
+    }
+    p.lse = lse_suffix; p.B = U * G; p.L = Lp + Ls; p.kv_end = kv_end;
+    p.G = G; p.Lp = Lp; p.Ls = Ls; p.sfx0 = (long long)U * Lp;
+    return launch<128, true, true>(tq, tk, tv, p, st);
 }

@@ -119,11 +119,14 @@ def _lin(x, w, *, lora_a=None, lora_b=None, lora_scale=1.0, saved_t=None, drop=N
 def decoder_forward(W: DecoderW, h: torch.Tensor, B: int, L: int, positions: torch.Tensor, kv_start, kv_end, *,
                     lora: Optional[LoraW] = None, saved: Optional[List[LayerSaved]] = None,
                     kv_sink: Optional[Callable[[int, torch.Tensor], None]] = None, final_norm: bool = True,
-                    dropout: Optional[LoraDropout] = None) -> torch.Tensor:
+                    dropout: Optional[LoraDropout] = None, layout=None) -> torch.Tensor:
     """Qwen3 decoder stack over dense rows [B, L] (HF qwen3/modeling_qwen3.py:294-336, 378-430).
 
     h: merged input embeddings [B*L, d] bf16 (not modified).  Returns the final-normed hidden states [B*L, d].
     dropout: LoRA dropout of this pass (only with `lora`); None runs the adapters undropped.
+    layout: optional training.SharedPrefixPlan: h, positions and the result are in its shared-prefix token buffer ([layout.N, d]) and
+    kv_start / kv_end are its per-group / per-row windows.  Only attention sees the layout (br_attn_fwd_shared); with `saved`, the
+    layer's lse is the (prefix, suffix) pair of segment buffers.
     """
     cfg = W.cfg
     Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
@@ -156,7 +159,14 @@ def decoder_forward(W: DecoderW, h: torch.Tensor, B: int, L: int, positions: tor
             q, k, v = qkv[:, qo:ko], qkv[:, ko:vo], qkv[:, vo:]
         if kv_sink is not None:
             kv_sink(li, qkv)
-        if S is not None:
+        if layout is not None:
+            res = ops.attn_fwd_shared(q, k, v, layout.U, layout.G, layout.Lp, layout.Ls, Hq, Hkv, D, kv_start, kv_end, want_lse=S is not None)
+            if S is not None:
+                attn, S.lse = res
+                S.attn = attn
+            else:
+                attn = res
+        elif S is not None:
             attn, lse = ops.attn_fwd(q, k, v, B, L, Hq, Hkv, D, kv_start=kv_start, kv_end=kv_end, causal=True, want_lse=True)
             S.attn, S.lse = attn, lse
         else:

@@ -250,6 +250,24 @@ def attn_fwd(q, k, v, B, L, n_q, n_kv, head_dim, *, kv_start=None, kv_end=None, 
     return (out, lse) if want_lse else out
 
 
+def attn_fwd_shared(q, k, v, U, G, Lp, Ls, n_q, n_kv, head_dim, kv_start, kv_end, *, scale=None, want_lse=False, out=None):
+    """Causal attention over the shared-prefix layout (br_attn_fwd_shared): q/k/v are 2-D views [U*Lp + U*G*Ls, heads*head_dim];
+    kv_start [U] per group, kv_end [U*G] per row.  Returns out (and (lse_prefix [U, Hq, Lp], lse_suffix [U*G, Hq, Ls]))."""
+    _need_cuda(q, k, v, kv_start, kv_end)
+    N = U * Lp + U * G * Ls
+    assert q.shape[0] == N and kv_start.dtype == torch.int32 and kv_end.dtype == torch.int32
+    if out is None:
+        out = torch.empty(N, n_q * head_dim, device=q.device, dtype=torch.bfloat16)
+    lse_p = torch.empty(U, n_q, Lp, device=q.device, dtype=torch.float32)
+    lse_s = torch.empty(U * G, n_q, Ls, device=q.device, dtype=torch.float32)
+    if scale is None:
+        scale = head_dim ** -0.5
+    check(lib().br_attn_fwd_shared(ptr(q), _row_major_2d(q), ptr(k), _row_major_2d(k), ptr(v), _row_major_2d(v), ptr(out), _row_major_2d(out),
+                                   ptr(lse_p, "float*"), ptr(lse_s, "float*"), U, G, Lp, Ls, n_q, n_kv, head_dim, ptr(kv_start, "int32_t*"),
+                                   ptr(kv_end, "int32_t*"), float(scale), _stream()), "attn_fwd_shared")
+    return (out, (lse_p, lse_s)) if want_lse else out
+
+
 # ------------------------------------------------------------------ decode
 def skinny_scratch(max_n: int, device) -> torch.Tensor:
     return torch.zeros(lib().br_skinny_scratch_bytes(max_n), device=device, dtype=torch.uint8)
@@ -347,6 +365,19 @@ def attn_bwd(q, k, v, o, dout, lse, dq, dk, dv, B, L, n_q, n_kv, head_dim, *, kv
                             ptr(dout), _row_major_2d(dout), ptr(lse, "float*"), ptr(dq), _row_major_2d(dq), ptr(dk), _row_major_2d(dk),
                             ptr(dv), _row_major_2d(dv), B, L, n_q, n_kv, head_dim, ptr(kv_start, "int32_t*"), ptr(kv_end, "int32_t*"),
                             float(scale), ptr(ws), _stream()), "attn_bwd")
+
+
+def attn_bwd_shared(q, k, v, o, dout, lse, dq, dk, dv, U, G, Lp, Ls, n_q, n_kv, head_dim, kv_start, kv_end, *, scale=None):
+    """Backward of attn_fwd_shared; lse = the (lse_prefix, lse_suffix) pair it returned."""
+    _need_cuda(q, k, v, o, dout, dq, dk, dv, kv_start, kv_end)
+    if scale is None:
+        scale = head_dim ** -0.5
+    lse_p, lse_s = lse
+    ws = torch.empty(lib().br_attn_bwd_shared_workspace_bytes(U, G, Lp, Ls, n_q, head_dim), device=q.device, dtype=torch.uint8)
+    check(lib().br_attn_bwd_shared(ptr(q), _row_major_2d(q), ptr(k), _row_major_2d(k), ptr(v), _row_major_2d(v), ptr(o), _row_major_2d(o),
+                                   ptr(dout), _row_major_2d(dout), ptr(lse_p, "float*"), ptr(lse_s, "float*"), ptr(dq), _row_major_2d(dq),
+                                   ptr(dk), _row_major_2d(dk), ptr(dv), _row_major_2d(dv), U, G, Lp, Ls, n_q, n_kv, head_dim,
+                                   ptr(kv_start, "int32_t*"), ptr(kv_end, "int32_t*"), float(scale), ptr(ws), _stream()), "attn_bwd_shared")
 
 
 def rmsnorm_bwd(x, w, rstd, dy, dres=None, out=None):

@@ -72,3 +72,4 @@ class DNALLMGRPOConfig:
     lora_alpha: float = 64.0
     micro_rows: Optional[int] = None      # rows per forward/backward chunk (None = as many as the device memory holds)
     suppress_eos: bool = False            # fixed-length rollouts (bench config c)
+    share_prompt_prefix: bool = False     # ref / old / policy passes compute each prompt group's full prompt tiles once (same log-probs)

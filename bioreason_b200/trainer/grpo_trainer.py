@@ -18,7 +18,7 @@ import torch
 import torch.distributed as dist
 from torch.utils.data import Sampler
 
-from .. import dp, ops, training
+from .. import dp, generation, ops, training
 from . import rewards as rw
 from .grpo_config import DNALLMGRPOConfig
 
@@ -110,6 +110,9 @@ class DNALLMGRPOTrainer:
             raise ValueError(f"The global train batch size ({world} x {a.per_device_train_batch_size}) must be evenly divisible by the "
                              f"number of generations per prompt ({self.num_generations}). Given the current train batch size, the valid "
                              f"values for the number of generations are: {possible}.")
+        if getattr(a, "share_prompt_prefix", False) and a.apply_lora_dropout:
+            raise ValueError("share_prompt_prefix cannot be combined with apply_lora_dropout: the dropout masks differ between the G copies "
+                             "of a prompt, so the prompt cannot be computed once")
         if model._lora is None:
             model.enable_lora(r=a.lora_r, alpha=a.lora_alpha, seed=a.seed)
         model.sync_adapters(rollout=True)
@@ -203,13 +206,21 @@ class DNALLMGRPOTrainer:
         return out
 
     # ------------------------------------------------------------------ log-probs
-    def _get_per_token_logps(self, model, input_ids, attention_mask, keep_last=None, lora="policy", dropout=False, **mm):
+    def _get_per_token_logps(self, model, input_ids, attention_mask, keep_last=None, lora="policy", dropout=False, group_size=None, **mm):
         """grpo_trainer.py:510-520 (+ the [:, P-1:] slice of :779 when keep_last is given), no-grad version."""
         n = input_ids.shape[1] - 1 if keep_last is None else keep_last
         with torch.no_grad():
             lp, _ = training.policy_forward(model, input_ids, attention_mask, mm.get("dna_tokenized"), mm.get("batch_idx_map"), n,
-                                            save=False, lora=lora, dropout=dropout)
+                                            save=False, lora=lora, dropout=dropout, **({"group_size": group_size} if group_size else {}))
         return lp
+
+    def _local_group_size(self, prompt_ids, mm) -> Optional[int]:
+        """Rows per prompt group in this rank's rows when share_prompt_prefix is on (None when off): consecutive identical prompts
+        (text and DNA), so a rank holding part of a group still shares it.  One host sync."""
+        if not getattr(self.args, "share_prompt_prefix", False):
+            return None
+        eq = generation.detect_group_size(prompt_ids, mm.get("dna_tokenized"), mm.get("batch_idx_map"))
+        return generation.group_size_from_flags([bool(x) for x in eq.tolist()])
 
     # ------------------------------------------------------------------ rollout + scoring
     @torch.no_grad()
@@ -238,10 +249,12 @@ class DNALLMGRPOTrainer:
         ids = torch.cat([prompt_ids, completion_ids], dim=1)
         attention_mask = torch.cat([prompt_mask, completion_mask.to(prompt_mask.dtype)], dim=1)                       # :612
         Cc = completion_ids.shape[1]
+        gs = self._local_group_size(prompt_ids, mm)
         with self._mark("ref_logps"):
             # the reference computes old log-probs in train mode: through the LoRA dropout when it is on
-            old_lp = self._get_per_token_logps(model, ids, attention_mask, keep_last=Cc, dropout=True, **mm) if self.num_iterations > 1 else None
-            ref_lp = self._get_per_token_logps(model, ids, attention_mask, keep_last=Cc, lora=None, **mm) if self.beta != 0.0 else None
+            old_lp = (self._get_per_token_logps(model, ids, attention_mask, keep_last=Cc, dropout=True, group_size=gs, **mm)
+                      if self.num_iterations > 1 else None)
+            ref_lp = self._get_per_token_logps(model, ids, attention_mask, keep_last=Cc, lora=None, group_size=gs, **mm) if self.beta != 0.0 else None
         # rewards: the reference protocol f(prompts=, completions=, **columns) on decoded text (:640-676); functions that name a
         # `completion_ids` parameter get device tensors instead (trainer/rewards.py)
         if rewards_per_func is None:
@@ -260,7 +273,8 @@ class DNALLMGRPOTrainer:
             self._metrics[f"rewards/{getattr(f, '__name__', 'reward_' + str(i))}"].append(rewards_all[:, i].mean())
         self.timings["score"] += time.perf_counter() - t0
         return dict(prompt_ids=prompt_ids, prompt_mask=prompt_mask, completion_ids=completion_ids, completion_mask=completion_mask,
-                    old_per_token_logps=old_lp, ref_per_token_logps=ref_lp, advantages=advantages, multimodal_inputs=mm)
+                    old_per_token_logps=old_lp, ref_per_token_logps=ref_lp, advantages=advantages, multimodal_inputs=mm,
+                    local_group_size=gs)
 
     @staticmethod
     def _auto_micro_rows(model, B, L):
@@ -272,6 +286,16 @@ class DNALLMGRPOTrainer:
         free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
         per_row = L * training.activation_bytes_per_token(model)
         return max(1, min(B, int(0.75 * free) // per_row))
+
+    @staticmethod
+    def _auto_micro_groups(model, U, G, P, L):
+        """Rows per chunk of the shared-prefix passes when `micro_rows` is open: whole groups, as many as fit like _auto_micro_rows,
+        a group costing Lp + G * Ls tokens of saved activations (one group per chunk when even one exceeds the estimate)."""
+        dev = model._dec.embed.device
+        free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+        Lp = training.SHARED_TILE * ((P - 1) // training.SHARED_TILE)
+        per_group = (Lp + G * (L - Lp)) * training.activation_bytes_per_token(model)
+        return G * max(1, min(U, int(0.75 * free) // per_group))
 
     # ------------------------------------------------------------------ loss (+ backward through the kernels)
     def compute_loss(self, model, inputs, return_outputs=False, num_items_in_batch=None, backward: bool = True):
@@ -291,7 +315,14 @@ class DNALLMGRPOTrainer:
         mask = torch.cat([prompt_mask, completion_mask.to(prompt_mask.dtype)], dim=1)
         B, C = completion_ids.shape
         adv, old, ref = inputs["advantages"], inputs["old_per_token_logps"], inputs["ref_per_token_logps"]
-        mr = self.args.micro_rows or (self._auto_micro_rows(model, B, ids.shape[1]) if ids.is_cuda else B)
+        gs = inputs["local_group_size"] if "local_group_size" in inputs else self._local_group_size(prompt_ids, mm)
+        if gs is not None and gs > 1:
+            # shared prompt prefix: chunks hold whole groups
+            if self.args.micro_rows and self.args.micro_rows % gs != 0:
+                raise ValueError(f"micro_rows ({self.args.micro_rows}) must be a multiple of the local group size ({gs}) with share_prompt_prefix")
+            mr = self.args.micro_rows or (self._auto_micro_groups(model, B // gs, gs, prompt_ids.shape[1], ids.shape[1]) if ids.is_cuda else B)
+        else:
+            mr = self.args.micro_rows or (self._auto_micro_rows(model, B, ids.shape[1]) if ids.is_cuda else B)
         ga = self.args.gradient_accumulation_steps
         loss_acc = torch.zeros(3, device=ids.device)
         # one LoRA-dropout pass for all row chunks; each chunk passes its first row so the masks ignore the chunking
@@ -304,7 +335,7 @@ class DNALLMGRPOTrainer:
             with self._mark("policy_fwd"):
                 drop_kw = dict(dropout=True, dropout_pass=pid, row_offset=lo) if pid is not None else {}
                 lp, ctx = training.policy_forward(model, ids[sl], mask[sl], mm_c["dna_tokenized"], mm_c["batch_idx_map"], C, save=backward,
-                                                  **drop_kw)
+                                                  **({"group_size": gs} if gs else {}), **drop_kw)
             out3, dlp = ops.grpo_loss_raw(lp, old[sl] if old is not None else None, ref[sl] if ref is not None else None, adv[sl],
                                           completion_mask[sl], self.beta, self.epsilon_low, self.epsilon_high, want_grad=backward)
             w = (hi - lo) / B

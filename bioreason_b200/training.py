@@ -7,6 +7,7 @@ is under no_grad in the reference (dna_llm.py:121).
 """
 from __future__ import annotations
 
+from dataclasses import dataclass
 from typing import List, Optional
 
 import torch
@@ -33,15 +34,78 @@ def activation_bytes_per_token(model) -> int:
     return cfg.num_hidden_layers * (bf16 + fp32) + 2 * d                   # + the final hidden state
 
 
+SHARED_TILE = 64          # tile height of the attention kernels: the shared prefix is a whole number of tiles
+
+
+@dataclass
+class SharedPrefixPlan:
+    """Shared-prefix token layout of U groups x G rows [prompt P | completion], L positions each (see plan_shared_prefix)."""
+    U: int
+    G: int
+    P: int
+    L: int
+    Lp: int                      # shared prefix length: positions 0 .. Lp-1 of a group are computed once
+    Ls: int                      # L - Lp positions per row suffix
+    N: int                       # buffer rows: U * Lp + U * G * Ls
+    src: torch.Tensor            # int32 [N]: dense row (r * L + t) each buffer row holds (the group's first row for prefix rows)
+    owner: torch.Tensor          # int32 [U*G*L]: buffer row of every dense row; -1 for the prefix positions of rows g > 0 of a group
+    positions: torch.Tensor      # int32 [N]: arange over the padded row
+    kv_start: torch.Tensor       # int32 [U]: attention window start of each group
+    kv_end: torch.Tensor         # int32 [U*G]: attention window end of each row
+    scored: torch.Tensor         # int32 [U*G*(L-P)]: buffer rows of positions P-1 .. L-2, row-major (the [B, L-P] log-prob order)
+
+    def owner_of(self, dense_rows: torch.Tensor) -> torch.Tensor:
+        """Buffer row owning each dense row index (-1 stays -1; prefix positions of rows g > 0 map to -1, so every (DNA feature,
+        destination) pair of the shared layout is counted once)."""
+        return torch.where(dense_rows >= 0, self.owner[dense_rows.clamp(min=0).long()], torch.full_like(dense_rows, -1)).to(torch.int32)
+
+
+def plan_shared_prefix(G: int, P: int, L: int, kv_start: torch.Tensor, kv_end: torch.Tensor) -> Optional[SharedPrefixPlan]:
+    """Shared-prefix layout of a batch of U = R / G groups whose G consecutive rows repeat one left-padded prompt of P columns,
+    followed by L - P completion positions (host side, pure; index bookkeeping only, on kv_end's device, no host sync).
+
+    The prefix is the prompt's full 64-position tiles minus one: Lp = 64 * floor((P - 1) / 64), so position P - 1 and every scored
+    position (P - 1 .. L - 2) lie in a row's own suffix; like the rollout's page plan, full tiles are shared and the tail is private.
+    Buffer rows: group u's positions 0 .. Lp-1 at u * Lp + t, row r = u * G + g's positions Lp + t at U * Lp + r * Ls + t.
+    kv_start / kv_end are the dense rows' windows (engine.mask_window); the rows of a group share kv_start, and every window ends past
+    the prefix (a completion follows the prompt).  Returns None (no sharing: the dense path) when G = 1 or Lp = 0."""
+    R = int(kv_end.numel())
+    if G <= 1 or R % G != 0 or P > L or P < 1:
+        return None
+    Lp = SHARED_TILE * ((P - 1) // SHARED_TILE)
+    if Lp <= 0:
+        return None
+    U, Ls = R // G, L - Lp
+    N = U * Lp + R * Ls
+    dev = kv_end.device
+    i64 = dict(device=dev, dtype=torch.long)
+    t_p, t_s = torch.arange(Lp, **i64), torch.arange(Ls, **i64)
+    u, r = torch.arange(U, **i64), torch.arange(R, **i64)
+    src = torch.cat([((u * G * L)[:, None] + t_p[None, :]).reshape(-1), ((r * L + Lp)[:, None] + t_s[None, :]).reshape(-1)])
+    owner = torch.full((R, L), -1, **i64)
+    owner[::G, :Lp] = (u * Lp)[:, None] + t_p[None, :]
+    owner[:, Lp:] = (U * Lp + r * Ls)[:, None] + t_s[None, :]
+    positions = torch.cat([t_p.repeat(U), (Lp + t_s).repeat(R)])
+    n = L - P
+    scored = ((U * Lp + r * Ls + (P - 1 - Lp))[:, None] + torch.arange(n, **i64)[None, :]).reshape(-1)
+    i32 = lambda x: x.to(torch.int32).contiguous()
+    return SharedPrefixPlan(U=U, G=G, P=P, L=L, Lp=Lp, Ls=Ls, N=N, src=i32(src), owner=i32(owner.reshape(-1)), positions=i32(positions),
+                            kv_start=i32(kv_start[::G]), kv_end=i32(kv_end), scored=i32(scored))
+
+
 def policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_map, keep_last: int, *, save: bool = True,
                    lora="policy", targets: Optional[torch.Tensor] = None, dropout: bool = False, dropout_pass: Optional[int] = None,
-                   row_offset: int = 0) -> "tuple[torch.Tensor, Optional[PolicyCtx]]":
+                   row_offset: int = 0, group_size: Optional[int] = None) -> "tuple[torch.Tensor, Optional[PolicyCtx]]":
     """Returns (logps [B, keep_last] fp32, ctx).  lora: "policy" (adapters on), None (base weights = reference policy).
     targets: optional [B, keep_last] class ids scored at the last keep_last positions before the end (default: the realised next
     tokens input_ids[:, L-keep_last:]); entries < 0 are ignored (log-prob 0, no gradient) -- the SFT label mask.
     dropout: apply the LoRA dropout set by `model.set_lora_dropout` (no-op while it is off or with lora=None).  Row chunks of one pass
     share `dropout_pass` (from `model.new_lora_dropout_pass()`; None draws a new pass) and give `row_offset` = the batch row of their
-    first row, so the masks do not depend on the chunking.  policy_backward regenerates the same masks from ctx."""
+    first row, so the masks do not depend on the chunking.  policy_backward regenerates the same masks from ctx.
+    group_size: G > 1 declares that every G consecutive rows repeat one prompt, the first L - keep_last columns (left-padded, as the GRPO
+    trainer builds them).  The decoder then runs on the shared-prefix layout (plan_shared_prefix): each group's full prompt tiles are
+    computed once.  The log-probs are the same, in the same [B, keep_last] order.  Not combinable with an active LoRA dropout (its masks
+    differ between the G copies of a prompt): ValueError."""
     W = model._dec
     dev = W.embed.device
     input_ids = input_ids.to(dev)
@@ -59,21 +123,34 @@ def policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_ma
     else:
         emb, aux = model.merged_embeddings(input_ids, dna_tokenized, batch_idx_map, return_proj_inputs=True)
     ks, ke = engine.mask_window(attention_mask)
-    pos = engine.forward_positions(B, L, dev)
     saved: Optional[List[LayerSaved]] = [] if save else None
     drop = None
     if dropout and use_lora is not None and model._lora.dropout is not None:
+        if group_size is not None and group_size > 1:
+            raise ValueError("group_size > 1 (shared prompt prefix) cannot be combined with LoRA dropout: its masks are drawn per token row, "
+                             "so the G copies of a prompt are not identical")
         pid = model._lora.new_dropout_pass() if dropout_pass is None else dropout_pass
         drop = model._lora.dropout_for(pid, row_offset * L)
-    h = engine.decoder_forward(W, emb, B, L, pos, ks, ke, lora=use_lora, saved=saved, final_norm=False, dropout=drop)
+    plan = plan_shared_prefix(group_size, L - keep_last, L, ks, ke) if group_size is not None and group_size > 1 else None
+    if plan is None:
+        pos = engine.forward_positions(B, L, dev)
+        h = engine.decoder_forward(W, emb, B, L, pos, ks, ke, lora=use_lora, saved=saved, final_norm=False, dropout=drop)
+    else:
+        pos = plan.positions
+        x = ops.gather_rows(emb, plan.src)                                 # the dense embeddings (DNA features included), prefix once
+        del emb
+        h = engine.decoder_forward(W, x, B, L, pos, plan.kv_start, plan.kv_end, lora=use_lora, saved=saved, final_norm=False, layout=plan)
     eps = W.cfg.rms_norm_eps
     if save:
         hn, rstd_f = ops.rmsnorm(h, W.final_norm, eps, want_rstd=True)
     else:
         hn, rstd_f = ops.rmsnorm(h, W.final_norm, eps), None
     n = keep_last
-    cols = torch.arange(L - 1 - n, L - 1, device=dev)
-    rows = (torch.arange(B, device=dev)[:, None] * L + cols[None, :]).reshape(-1).to(torch.int32)
+    if plan is None:
+        cols = torch.arange(L - 1 - n, L - 1, device=dev)
+        rows = (torch.arange(B, device=dev)[:, None] * L + cols[None, :]).reshape(-1).to(torch.int32)
+    else:
+        rows = plan.scored
     h_sel = ops.gather_rows(hn, rows)
     tgt = (input_ids[:, L - n:] if targets is None else targets.to(dev)).reshape(-1).to(torch.int32)
     logp, lse = ops.lmhead_logprob(h_sel, W.lm_head, tgt)
@@ -86,6 +163,7 @@ def policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_ma
         ctx.pos, ctx.ks, ctx.ke, ctx.aux = pos, ks, ke, aux
         ctx.use_lora = use_lora is not None
         ctx.drop = drop
+        ctx.layout = plan
     return logp.view(B, n), ctx
 
 
@@ -101,7 +179,8 @@ def policy_backward(model, ctx: PolicyCtx, dlogp: torch.Tensor, on_layer_done=No
     theta = cfg.rope_parameters["rope_theta"] if hasattr(cfg, "rope_parameters") else cfg.rope_theta
     eps = cfg.rms_norm_eps
     B, L = ctx.B, ctx.L
-    M = B * L
+    layout = getattr(ctx, "layout", None)
+    M = B * L if layout is None else layout.N
     dev = W.embed.device
     lora = model._lora if ctx.use_lora else None
     r = lora.r if lora else 0
@@ -165,8 +244,12 @@ def policy_backward(model, ctx: PolicyCtx, dlogp: torch.Tensor, on_layer_done=No
         else:
             dattn = ops.gemm(dh_mid, Lw.w_o_T)
         dqkv = torch.empty(M, (Hq + 2 * Hkv) * D, device=dev, dtype=torch.bfloat16)
-        ops.attn_bwd(S.q, S.k, S.v, S.attn, dattn, S.lse, dqkv[:, qo:ko], dqkv[:, ko:vo], dqkv[:, vo:],
-                     B, L, Hq, Hkv, D, kv_start=ctx.ks, kv_end=ctx.ke)
+        if layout is None:
+            ops.attn_bwd(S.q, S.k, S.v, S.attn, dattn, S.lse, dqkv[:, qo:ko], dqkv[:, ko:vo], dqkv[:, vo:],
+                         B, L, Hq, Hkv, D, kv_start=ctx.ks, kv_end=ctx.ke)
+        else:
+            ops.attn_bwd_shared(S.q, S.k, S.v, S.attn, dattn, S.lse, dqkv[:, qo:ko], dqkv[:, ko:vo], dqkv[:, vo:], layout.U, layout.G,
+                                layout.Lp, layout.Ls, Hq, Hkv, D, layout.kv_start, layout.kv_end)
         del dattn
         ops.qk_rope_bwd_(dqkv, S.qkv_pre, Hq, Hkv, D, Lw.q_norm, Lw.k_norm, ctx.pos, theta, eps)
         if lora:
@@ -188,6 +271,10 @@ def policy_backward(model, ctx: PolicyCtx, dlogp: torch.Tensor, on_layer_done=No
     # ---------------- projector: emb rows that came from DNA features
     if ctx.aux is not None and model.dna_projection.weight.requires_grad:
         enc, row_map = ctx.aux
+        if layout is not None:
+            # each (feature, buffer row) pair once: a prefix row carries the gradient of the whole group and is owned by the group's
+            # first row; a tail feature of every row lands in that row's suffix
+            row_map = layout.owner_of(row_map)
         dE = ops.gather_rows(dh, row_map)                                  # rows with row_map < 0 (DNA pads) come back as zeros
         dE_T = ops.transpose(dE)                                           # [d_text, n']
         enc_T = ops.transpose(enc)                                         # [d_dna, n']

@@ -137,6 +137,15 @@ int br_gather_rows(const void* src, int64_t lds, const int32_t* idx, void* dst, 
 int br_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o, int64_t ldo,
                 float* lse, int B, int L, int n_q_heads, int n_kv_heads, int head_dim, const int32_t* kv_start,
                 const int32_t* kv_end, float scale, int causal, void* stream);
+/* Shared-prefix layout (GRPO groups: G rows that repeat one prompt): U groups of G rows of L = Lp + Ls positions, Lp a multiple of 64.
+ * The buffer holds [U * Lp prefix rows | R = U * G suffixes of Ls rows]: group u's positions 0 .. Lp-1 are rows u * Lp + t, row
+ * r = u * G + g's position Lp + t is row U * Lp + r * Ls + t.  Causal, head_dim 128; kv_start [U] per group (the rows of a group share
+ * their prompt), kv_end [R] per row, with kv_end >= Lp (every row's window reaches past the prefix).  The log-sum-exp is kept as two
+ * segment buffers: lse_prefix [U, Hq, Lp] (unused when Lp = 0) and lse_suffix [R, Hq, Ls].  O and the log-sum-exp are bit-identical
+ * to br_attn_fwd on the equivalent dense [R, L] rows. */
+int br_attn_fwd_shared(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o, int64_t ldo,
+                       float* lse_prefix, float* lse_suffix, int U, int G, int Lp, int Ls, int n_q_heads, int n_kv_heads, int head_dim,
+                       const int32_t* kv_start, const int32_t* kv_end, float scale, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Rollout / decode (replaces the HF generate() token loop, DynamicCache and logits warpers reached from
@@ -200,6 +209,14 @@ int br_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const vo
                 const void* dout, int64_t lddo, const float* lse, void* dq, int64_t lddq, void* dk, int64_t lddk, void* dv,
                 int64_t lddv, int B, int L, int n_q_heads, int n_kv_heads, int head_dim, const int32_t* kv_start,
                 const int32_t* kv_end, float scale, void* workspace, void* stream);
+/* Backward of br_attn_fwd_shared (same layout and windows).  dQ of every query and dK / dV of the suffix keys are bit-identical to
+ * br_attn_bwd on the dense rows; the prefix dK / dV sum the group's prefix queries, then the queries of rows g = 0 .. G-1 in that order
+ * (bit-identical to the dense result when G = 1).  No atomics: bit-reproducible.  workspace: br_attn_bwd_shared_workspace_bytes. */
+int64_t br_attn_bwd_shared_workspace_bytes(int U, int G, int Lp, int Ls, int n_q_heads, int head_dim);
+int br_attn_bwd_shared(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const void* o, int64_t ldo,
+                       const void* dout, int64_t lddo, const float* lse_prefix, const float* lse_suffix, void* dq, int64_t lddq, void* dk,
+                       int64_t lddk, void* dv, int64_t lddv, int U, int G, int Lp, int Ls, int n_q_heads, int n_kv_heads, int head_dim,
+                       const int32_t* kv_start, const int32_t* kv_end, float scale, void* workspace, void* stream);
 /* dx = d(RMSNorm)/dx . dy (+ dres): x, dy, dres, dx bf16 [M, d]; rstd from the forward */
 int br_rmsnorm_bwd(const void* x, int64_t ldx, const void* w, const float* rstd, const void* dy, int64_t lddy, const void* dres,
                    int64_t lddr, void* dx, int64_t lddx, int M, int d, void* stream);
