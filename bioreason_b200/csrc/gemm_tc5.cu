@@ -3,11 +3,13 @@
 // Replaces every nn.Linear / lm_head matmul the reference reaches through HF (SURVEY.md §2.3 K1,K2,K5,K6,K12):
 // both operands are K-major (nn.Linear weight layout [out, in]), bf16 in, fp32 accumulate in registers.
 //
-// Structure (one persistent CTA per SM, 288 threads):
-//   warp 8      TMA producer   : cp.async.bulk.tensor 2-D, 128B-swizzled 128x64 (A) and 128x64 (B) tiles, NSTAGE ring
-//   warps 0..7  two consumer warpgroups: each issues wgmma.mma_async m64n128k16 for its 64 rows of the 128 x 128 tile (one
+// Structure (one persistent CTA per SM, 288 threads, a 128 x BN tile with BN = 128 or 256 chosen per problem in run_gemm):
+//   warp 8      TMA producer   : cp.async.bulk.tensor 2-D, 128B-swizzled 128x64 (A) and BNx64 (B) tiles, NSTAGE ring
+//   warps 0..7  two consumer warpgroups: each issues wgmma.mma_async m64nBNk16 for its 64 rows of the 128 x BN tile (one
 //                                wgmma group kept in flight; a stage goes back to the producer as soon as its products retire),
 //                                then runs the fused epilogue straight from the register fragment
+// Every output element accumulates over K in the same k16 order at either width, and the epilogues round at the same points, so
+// the two tile widths give bit-identical results.
 // LoRA dropout (MASK): the second K segment u . A of the dX GEMM is formed one projection (r-wide K block) at a time in a temporary
 // accumulator, multiplied by that projection's counter-based mask and 1 / (1 - p_eff) in registers, and added to the main accumulator
 // before the usual epilogue (one rounding, no extra HBM traffic).
@@ -21,7 +23,6 @@
 namespace {
 
 constexpr int BM = 128;
-constexpr int BN = 128;
 constexpr int BK = 64;
 constexpr int NTHREADS = 288;
 
@@ -42,16 +43,18 @@ struct GemmParams {
     const int* target;       // [M] class index per row (or <0)
     float* pmax; float* psum; float* tgt_logit;   // [M, n_tiles_n], [M, n_tiles_n], [M]
     const float* lse; const float* gscale;        // [M]
-    int n_tiles_m, n_tiles_n;
+    int n_tiles_m, n_tiles_n;      // 128-row and 128-column tiles; a BN-wide tile spans BN / 128 column tiles
+                                   // (MODE_LSE writes one partial per 128-column tile: [M, n_tiles_n])
     int group_m;             // m-blocks per raster group (see tile_coords)
     br::DropParams drop;     // MASK: dropout of the second segment's projections
 };
 
+template <int BN>
 struct SmemLayout {
     static constexpr int A_BYTES = BM * BK * 2;
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int NSTAGE = 6;                        // 6 x 32 KB of the 227 KB a block may use
+    static constexpr int NSTAGE = BN == 128 ? 6 : 4;        // 6 x 32 KB or 4 x 48 KB of the 227 KB a block may use
     static constexpr int TILE_BYTES = NSTAGE * STAGE_BYTES;
     static constexpr int TOTAL = TILE_BYTES + 256 + 1024;   // + barriers + alignment slack
 };
@@ -72,6 +75,7 @@ __device__ __forceinline__ float rbf(float x) { return __bfloat162float(__float2
 
 // One BK block of the LoRA segment under dropout: for each projection whose r-wide K slice lies in the block, tmp = u_j . A_j (its k16
 // steps), then acc += m_j * inv_keep * tmp over the thread's fragment.  Retires every outstanding wgmma of the tile first.
+template <int BN>
 __device__ __forceinline__ void masked_segment(float (&acc)[BN / 2], uint64_t adesc, uint64_t bdesc, int k0, int mb, int nb, int wg,
                                                const GemmParams& p) {
     const int lane = threadIdx.x & 31, q = lane & 3;
@@ -109,12 +113,15 @@ __device__ __forceinline__ void masked_segment(float (&acc)[BN / 2], uint64_t ad
     }
 }
 
-template <int MODE, bool MASK>
+template <int BN, int MODE, bool MASK>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
                 const GemmParams p) {
-    using L = SmemLayout;
+    static_assert(BN == 128 || BN == 256, "tile width");
+    static_assert(!MASK || BN == 128, "the masked LoRA segment runs on 128-wide tiles");
+    constexpr int NSUB = BN / 128;                          // 128-column tiles per tile
+    using L = SmemLayout<BN>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::TILE_BYTES);
@@ -122,7 +129,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int num_tiles = p.n_tiles_m * p.n_tiles_n;
+    const int num_tiles = p.n_tiles_m * ((p.n_tiles_n + NSUB - 1) / NSUB);
     const int kb1 = (p.K + BK - 1) / BK;
     const int kb2 = (p.K2 + BK - 1) / BK;
     const int num_kb = kb1 + kb2;
@@ -141,7 +148,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         if (lane == 0) {
             int s = 0; uint32_t ph = 0;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                int mb, nb; tile_coords(tile, p.n_tiles_m, p.n_tiles_n, p.group_m, mb, nb);
+                int mb, nb; tile_coords(tile, p.n_tiles_m, (p.n_tiles_n + NSUB - 1) / NSUB, p.group_m, mb, nb);
                 for (int kb = 0; kb < num_kb; ++kb) {
                     br::mbar_wait(&empty_bar[s], ph ^ 1);
                     uint8_t* sa = smem + s * L::STAGE_BYTES;
@@ -165,7 +172,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     const int wt = threadIdx.x & 127;
     int s = 0; uint32_t ph = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int mb, nb; tile_coords(tile, p.n_tiles_m, p.n_tiles_n, p.group_m, mb, nb);
+        int mb, nb; tile_coords(tile, p.n_tiles_m, (p.n_tiles_n + NSUB - 1) / NSUB, p.group_m, mb, nb);
         float acc[BN / 2];
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -177,7 +184,7 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             const uint64_t bdesc = br::wg_desc_k(sa + L::A_BYTES);
             if constexpr (MASK) {
                 if (kb >= kb1) {
-                    masked_segment(acc, adesc, bdesc, (kb - kb1) * BK, mb, nb, wg, p);
+                    masked_segment<BN>(acc, adesc, bdesc, (kb - kb1) * BK, mb, nb, wg, p);
                     if (wt == 0) br::mbar_arrive(&empty_bar[prev]);       // masked_segment retired every product: release the previous stage
                     prev = s;
                     if (++s == L::NSTAGE) { s = 0; ph ^= 1; }
@@ -263,33 +270,39 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                 }
             }
         } else if constexpr (MODE == MODE_LSE) {
-            // per-row max / sum-exp over this tile's columns (the four lanes of a quad share a row) + target-logit pick
+            // per-row max / sum-exp over each 128-column tile (the four lanes of a quad share a row) + target-logit pick.  A 256-wide
+            // tile writes its two halves as two partials, so the partials and their combine do not depend on the tile width.
 #pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-                const int row = r0 + 8 * hh;
-                const bool row_ok = row < p.M;
-                const int tgt = row_ok ? p.target[row] : -1;
-                float mx = -INFINITY;
+            for (int h = 0; h < NSUB; ++h) {
+                const int nh = n0 + 128 * h;
+                if (NSUB > 1 && nh >= p.N) break;           // the last 256-wide tile may cover a single 128-column tile
 #pragma unroll
-                for (int i = 0; i < BN / 8; ++i)
-                    if (n0 + 8 * i < p.N) mx = fmaxf(mx, fmaxf(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]) * p.alpha);
-                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-                float sm = 0.f;
+                for (int hh = 0; hh < 2; ++hh) {
+                    const int row = r0 + 8 * hh;
+                    const bool row_ok = row < p.M;
+                    const int tgt = row_ok ? p.target[row] : -1;
+                    float mx = -INFINITY;
 #pragma unroll
-                for (int i = 0; i < BN / 8; ++i) {
-                    if (n0 + 8 * i >= p.N) continue;
-                    const int col = n0 + 8 * i + cq;
-                    const float x0 = acc[4 * i + 2 * hh] * p.alpha, x1 = acc[4 * i + 2 * hh + 1] * p.alpha;
-                    sm += __expf(x0 - mx) + __expf(x1 - mx);
-                    if (col == tgt) p.tgt_logit[row] = x0;
-                    if (col + 1 == tgt) p.tgt_logit[row] = x1;
-                }
-                sm += __shfl_xor_sync(0xffffffffu, sm, 1);
-                sm += __shfl_xor_sync(0xffffffffu, sm, 2);
-                if (row_ok && (lane & 3) == 0) {
-                    p.pmax[(long long)row * p.n_tiles_n + nb] = mx;
-                    p.psum[(long long)row * p.n_tiles_n + nb] = sm;
+                    for (int i = 0; i < 16; ++i)
+                        if (nh + 8 * i < p.N) mx = fmaxf(mx, fmaxf(acc[64 * h + 4 * i + 2 * hh], acc[64 * h + 4 * i + 2 * hh + 1]) * p.alpha);
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                    float sm = 0.f;
+#pragma unroll
+                    for (int i = 0; i < 16; ++i) {
+                        if (nh + 8 * i >= p.N) continue;
+                        const int col = nh + 8 * i + cq;
+                        const float x0 = acc[64 * h + 4 * i + 2 * hh] * p.alpha, x1 = acc[64 * h + 4 * i + 2 * hh + 1] * p.alpha;
+                        sm += __expf(x0 - mx) + __expf(x1 - mx);
+                        if (col == tgt) p.tgt_logit[row] = x0;
+                        if (col + 1 == tgt) p.tgt_logit[row] = x1;
+                    }
+                    sm += __shfl_xor_sync(0xffffffffu, sm, 1);
+                    sm += __shfl_xor_sync(0xffffffffu, sm, 2);
+                    if (row_ok && (lane & 3) == 0) {
+                        p.pmax[(long long)row * p.n_tiles_n + nb * NSUB + h] = mx;
+                        p.psum[(long long)row * p.n_tiles_n + nb * NSUB + h] = sm;
+                    }
                 }
             }
         } else {
@@ -346,19 +359,27 @@ PFN_encodeTiled get_encode() {
     return fn;
 }
 
-template <int MODE, bool MASK = false>
+template <int BN, int MODE, bool MASK = false>
 int launch(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& a2, const CUtensorMap& b2, const GemmParams& p, cudaStream_t st) {
-    auto kern = gemm_tc5_kernel<MODE, MASK>;
+    auto kern = gemm_tc5_kernel<BN, MODE, MASK>;
     static bool attr_set = false;
     if (!attr_set) {
-        BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemLayout::TOTAL));
+        BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemLayout<BN>::TOTAL));
         attr_set = true;
     }
-    int tiles = p.n_tiles_m * p.n_tiles_n;
+    int tiles = p.n_tiles_m * ((p.n_tiles_n + BN / 128 - 1) / (BN / 128));
     int grid = tiles < br_num_sms() ? tiles : br_num_sms();
-    kern<<<grid, NTHREADS, SmemLayout::TOTAL, st>>>(a, b, a2, b2, p);
+    kern<<<grid, NTHREADS, SmemLayout<BN>::TOTAL, st>>>(a, b, a2, b2, p);
     BR_CHECK_LAUNCH();
     return BR_OK;
+}
+
+template <int BN>
+int launch_mode(int mode, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& a2, const CUtensorMap& b2, const GemmParams& p,
+                cudaStream_t st) {
+    if (mode == MODE_STD) return launch<BN, MODE_STD>(a, b, a2, b2, p, st);
+    if (mode == MODE_LSE) return launch<BN, MODE_LSE>(a, b, a2, b2, p, st);
+    return launch<BN, MODE_DLOGITS>(a, b, a2, b2, p, st);
 }
 
 int run_gemm(int mode, const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, const void* A2, int64_t lda2,
@@ -368,8 +389,21 @@ int run_gemm(int mode, const void* A, int64_t lda, const void* B, int64_t ldb, i
     BR_CHECK_ARG(((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0), "gemm: operands must be 16-byte aligned");
     p.M = M; p.N = N; p.K = K; p.K2 = (A2 && B2) ? K2 : 0;
     p.n_tiles_m = (M + BM - 1) / BM;
-    p.n_tiles_n = (N + BN - 1) / BN;
-    {   // A panel of one raster group ~ 16 MB of the 50 MB L2 (the concurrently streaming B panels and the outputs need the rest)
+    p.n_tiles_n = (N + 127) / 128;
+    // Tile width.  Per k16, each warpgroup reads its A slice and the whole B slice from shared memory; m64n256 does twice the math
+    // of m64n128 for the same A read, and a 256-wide CTA loads each A tile from L2 once per 256 output columns instead of once per
+    // 128 (1.1-1.3x the TFLOP/s on the training shapes, DESIGN.md section 5).  The 128 x 256 tile has half as many tiles to spread over the SMs and a 4-stage ring, so it is used only where the
+    // tiles still fill two waves of the persistent grid and the main loop dominates the tile: N >= 256, K >= 512 and at least
+    // 2 x SMs 256-wide tiles.  That takes the training-pass linears at the trainer's chunk sizes (4 x 2364 dense rows, 6368
+    // shared-prefix rows) and the lm_head.  The LoRA down / up products (N = r x projections <= 96), the merged-weight rebuild
+    // (K = r), the DNA encoder, the projector and one-prompt prefills of the 2560-wide outputs keep 128 x 128.  The masked LoRA
+    // segment (dropout) always runs 128-wide: it needs a second accumulator of the tile's width.
+    const bool wide = !masked && N >= 256 && K >= 512 && (long long)p.n_tiles_m * ((N + 255) / 256) >= 2ll * br_num_sms();
+    const int bn = wide ? 256 : 128;
+    {   // A panel of one raster group ~ 16 MB of the 50 MB L2 (the concurrently streaming B panels and the outputs need the rest).
+        // The rule counts 128-row A blocks, so it is the same at both tile widths: B is re-read from DRAM once per group at either
+        // width, and the B panels of one wave of 256-wide tiles, (SMs / group_m) x 256 x K x 2 bytes, stay within the rest of L2 up
+        // to K = 4096 (beyond that, at N = 2560 the whole of B is live at either width).
         const long long a_block = (long long)BM * (K + p.K2) * 2;
         long long g = (16ll << 20) / (a_block > 0 ? a_block : 1);
         if (g < 8) g = 8;
@@ -379,16 +413,14 @@ int run_gemm(int mode, const void* A, int64_t lda, const void* B, int64_t ldb, i
     CUtensorMap ta, tb, ta2, tb2;
     int rc;
     if ((rc = br_make_tmap_2d_bf16(&ta, A, M, K, lda, BM))) return rc;
-    if ((rc = br_make_tmap_2d_bf16(&tb, B, N, K, ldb, BN))) return rc;
+    if ((rc = br_make_tmap_2d_bf16(&tb, B, N, K, ldb, bn))) return rc;
     if (p.K2) {
         BR_CHECK_ARG(K2 % 8 == 0 && lda2 % 8 == 0 && ldb2 % 8 == 0, "gemm: K2, lda2, ldb2 must be multiples of 8");
         if ((rc = br_make_tmap_2d_bf16(&ta2, A2, M, K2, lda2, BM))) return rc;
-        if ((rc = br_make_tmap_2d_bf16(&tb2, B2, N, K2, ldb2, BN))) return rc;
+        if ((rc = br_make_tmap_2d_bf16(&tb2, B2, N, K2, ldb2, bn))) return rc;
     } else { ta2 = ta; tb2 = tb; }
-    if (masked) return launch<MODE_STD, true>(ta, tb, ta2, tb2, p, st);
-    if (mode == MODE_STD) return launch<MODE_STD>(ta, tb, ta2, tb2, p, st);
-    if (mode == MODE_LSE) return launch<MODE_LSE>(ta, tb, ta2, tb2, p, st);
-    return launch<MODE_DLOGITS>(ta, tb, ta2, tb2, p, st);
+    if (masked) return launch<128, MODE_STD, true>(ta, tb, ta2, tb2, p, st);
+    return wide ? launch_mode<256>(mode, ta, tb, ta2, tb2, p, st) : launch_mode<128>(mode, ta, tb, ta2, tb2, p, st);
 }
 
 }  // namespace
@@ -443,7 +475,7 @@ int br_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ldb, void* D
 }
 
 int64_t br_lmhead_workspace_bytes(int M, int V) {
-    int nt = (V + 127) / 128;   // BN = 128
+    int nt = (V + 127) / 128;   // one (max, sum-exp) partial per 128-column tile at either tile width
     return (int64_t)M * nt * 2 * sizeof(float) + (int64_t)M * sizeof(float);
 }
 

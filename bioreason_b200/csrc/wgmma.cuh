@@ -35,6 +35,7 @@ __device__ __forceinline__ void wg_fence_operand(float (&d)[N]) {
 #define BR_WG_F16(i) BR_WG_F8(i), BR_WG_F8(i + 8)
 #define BR_WG_F32(i) BR_WG_F16(i), BR_WG_F16(i + 16)
 #define BR_WG_F64(i) BR_WG_F32(i), BR_WG_F32(i + 32)
+#define BR_WG_F128(i) BR_WG_F64(i), BR_WG_F64(i + 64)
 
 template <int N, int TA, int TB> struct WgSS;
 template <int N, int TB> struct WgRS;
@@ -65,6 +66,13 @@ template <int TA, int TB> struct WgSS<128, TA, TB> {      // D[64 x 128] (+)= A[
         asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
                      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n}\n"
                      : BR_WG_F64(0) : "l"(a), "l"(b), "r"(accumulate), "n"(TA), "n"(TB));
+    }
+};
+template <int TA, int TB> struct WgSS<256, TA, TB> {      // D[64 x 256] (+)= A[64 x 16] . B[16 x 256]; TA / TB = 1: MN-major operand
+    static __device__ __forceinline__ void run(float (&d)[128], uint64_t a, uint64_t b, int accumulate) {
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+                     "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n}\n"
+                     : BR_WG_F128(0) : "l"(a), "l"(b), "r"(accumulate), "n"(TA), "n"(TB));
     }
 };
 template <int TB> struct WgRS<16, TB> {                 // D[64 x 16] (+)= A[64 x 16] (registers) . B[16 x 16] (shared memory)
@@ -99,6 +107,7 @@ template <int TB> struct WgRS<128, TB> {                 // D[64 x 128] (+)= A[6
 #undef BR_WG_F16
 #undef BR_WG_F32
 #undef BR_WG_F64
+#undef BR_WG_F128
 
 template <int N, int TA = 0, int TB = 0>
 __device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t a, uint64_t b, int accumulate) { WgSS<N, TA, TB>::run(d, a, b, accumulate); }
