@@ -8,6 +8,7 @@ prefilled once and share their prompt KV pages.
 """
 from __future__ import annotations
 
+import gc
 import math
 from dataclasses import dataclass
 from types import SimpleNamespace
@@ -317,8 +318,17 @@ class RolloutEngine:
                     t.copy_(v)                                                # the warm-up step is replayed for real below
                 St.graph = torch.cuda.CUDAGraph()
                 n0 = ops.LAUNCHES[0]
-                with torch.cuda.graph(St.graph):
-                    decode_step()
+                # A dropped model and its engine reference each other, so their captured graphs live until the cyclic collector
+                # runs, and destroying a graph while a stream captures invalidates the capture: collect now, not inside the capture.
+                gc_was_enabled = gc.isenabled()
+                gc.collect()
+                gc.disable()
+                try:
+                    with torch.cuda.graph(St.graph):
+                        decode_step()
+                finally:
+                    if gc_was_enabled:
+                        gc.enable()
                 St.per_replay = ops.LAUNCHES[0] - n0
                 ops.LAUNCHES[0] = n0
                 for t, v in zip((tokens, next_ids, finished, step, cur_len), state):

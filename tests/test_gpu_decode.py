@@ -339,6 +339,41 @@ def test_generate_eos_and_multi_group(golden, tiny_oracle):
     _first_mismatch_ok(got.cpu(), want, margins, tol=0.02)
 
 
+def test_decode_capture_is_safe_from_the_cyclic_collector(golden, tiny_oracle, monkeypatch):
+    """A model and its rollout engine reference each other, so a dropped model's captured decode graph lives until Python's cyclic
+    collector runs, and destroying a graph while a stream captures invalidates that capture.  generate() must free such garbage
+    before it captures and keep the collector off during the capture (a collection there once broke the next rollout, depending on
+    how many objects earlier tests had allocated)."""
+    import gc
+    import weakref
+    from bioreason_b200.models import DNALLMModel
+    D = golden["D"]
+    old = DNALLMModel.from_oracle(tiny_oracle)
+    old.generate(**D["batch"], max_new_tokens=12, do_sample=False)
+    assert old._rollout._cached, "the first rollout captured a decode graph"
+    probe = weakref.ref(old._rollout)
+    was_enabled = gc.isenabled()
+    gc.disable()
+    try:
+        del old
+        assert probe() is not None, "the model / engine cycle keeps the captured graph alive after the model is dropped"
+    finally:
+        if was_enabled:
+            gc.enable()
+    seen = []
+    enter = torch.cuda.graph.__enter__
+
+    def spy(self):
+        seen.append((gc.isenabled(), probe() is None))
+        return enter(self)
+    monkeypatch.setattr(torch.cuda.graph, "__enter__", spy)
+    m = DNALLMModel.from_oracle(tiny_oracle)
+    got = m.generate(**D["batch"], max_new_tokens=12, do_sample=False).cpu()
+    assert seen == [(False, True)], "capture must start with the collector off and the dropped engine (and its graph) freed"
+    assert gc.isenabled() == was_enabled
+    assert torch.equal(got, m.generate(**D["batch"], max_new_tokens=12, do_sample=False, use_graph=False).cpu())
+
+
 def test_generate_ignores_recycled_allocator_garbage(golden, tiny_oracle):
     """Buffers of a rollout come from torch's caching allocator, i.e. they may hold anything -- including NaN bit patterns -- that an
     earlier tensor left behind.  Masked positions are multiplied by exact-zero probabilities, which is only harmless for finite
