@@ -100,6 +100,13 @@ __device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const void* tma
         "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(policy)
         : "memory");
 }
+// contiguous bulk copy global -> shared (bytes and both addresses 16-byte aligned), same completion and hint as above
+__device__ __forceinline__ void bulk_load_hint(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t policy) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(smem_u32(smem_dst)),
+        "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+        : "memory");
+}
 __device__ __forceinline__ uint64_t make_policy_evict_first() {
     uint64_t p; asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p)); return p;
 }

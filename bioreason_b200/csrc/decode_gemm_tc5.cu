@@ -14,12 +14,17 @@
 //     is reduced deterministically: every contributor writes its fp32 partial tile to its own scratch slot, the last arriver
 //     (arrival counter) sums the slots in ascending CTA order and applies the epilogue -- no floating-point atomics.
 // Epilogues: bf16 store, +residual, SwiGLU over (8 gate | 8 up) feature blocks, fp32 logits.
+// Weight format (template parameter FP8): bf16 tiles by 2-D TMA (128B swizzle, both wgmma operands in shared memory), or e4m3 units
+// (fp8_weights.cuh: 8 KB per 128x64 unit, one bulk copy, fragment order) that the consumer converts exactly to the bf16 register-A
+// operand; the per-row fp32 scale multiplies the finished accumulator before the epilogue.  Half the bytes per stage buys a deeper
+// ring in the same shared memory.
 // PDL: the kernel is launched with programmatic stream serialization.  Kernels chained this way are NOT separated by the
 // usual launch-boundary L1 invalidation, so every load of data another kernel of the chain rewrites (residual, statistics,
 // scratch) goes through L2 (ld.global.cg / TMA), never through L1.
 #include "br_common.cuh"
 #include "../../include/bioreason_b200.h"
 #include "wgmma.cuh"
+#include "fp8_weights.cuh"
 
 namespace {
 
@@ -37,17 +42,19 @@ struct SkParams {
     // columns); sumsq_out[(tile*4 + warp), r] = sum over that warp's 32 features of out[r, f]^2 (bf16-rounded) -- partials are
     // written, never accumulated with atomics, and summed in a fixed order by the consumer: the rollout is reproducible.
     const float* sumsq_in; int sumsq_in_n; float* sumsq_out; float eps;
+    const uint8_t* wq; const float* wscale;   // FP8 weights: e4m3 units (fp8_weights.cuh) and the per-row scales
 };
 
 __device__ __forceinline__ float rbf(float x) { return __bfloat162float(__float2bfloat16(x)); }
 
 
-template <int BNX>
+template <int BNX, bool FP8 = false>
 struct SL {
-    static constexpr int A_BYTES = BM * BK * 2;
+    static constexpr int A_BYTES = FP8 ? br::fp8w::UNIT_BYTES : BM * BK * 2;
     static constexpr int B_BYTES = BNX * BK * 2;
     static constexpr int STAGE = A_BYTES + B_BYTES;
-    static constexpr int NSTAGE = BNX == 16 ? 5 : 4;         // <= 101 KB per CTA: this kernel and its PDL successor fit one SM (228 KB)
+    // <= 101 KB per CTA: this kernel and its PDL successor fit one SM (228 KB)
+    static constexpr int NSTAGE = FP8 ? (BNX == 16 ? 9 : 6) : (BNX == 16 ? 5 : 4);
     static constexpr int TILE_BYTES = NSTAGE * STAGE;
     static constexpr int TR_BYTES = BM * (BNX + 1) * 4;       // accumulator transpose: one feature row per epilogue thread
     static constexpr int TOTAL = TILE_BYTES + TR_BYTES + 1024 + 1024;   // + barriers / flags / per-row rstd + alignment slack
@@ -56,10 +63,10 @@ struct SL {
 // The accumulator of one 128-feature tile over `n_units` consecutive ring stages (swap-AB: the weight tile is the M operand of two
 // m64nBNXk16 wgmma products, the X tile the N operand), then transposed through shared memory so that thread et holds feature et of
 // the tile for every row (the layout the epilogue and the stream-K exchange work in).  Called by the consumer warpgroup (warps 0..3).
-template <int BNX, int RM>
+template <int BNX, int RM, bool FP8>
 __device__ __forceinline__ void mma_tile(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, int& s, uint32_t& ph, int n_units,
                                          float* s_tr, float (&v)[RM]) {
-    using L = SL<BNX>;
+    using L = SL<BNX, FP8>;
     const int et = threadIdx.x, warp = et >> 5, lane = et & 31;
     float acc0[BNX / 2], acc1[BNX / 2];
 #pragma unroll
@@ -68,11 +75,30 @@ __device__ __forceinline__ void mma_tile(uint8_t* smem, uint64_t* full_bar, uint
         br::mbar_wait(&full_bar[s], ph);
         const uint32_t sa = br::smem_u32(smem + s * L::STAGE);
         const uint64_t bdesc = br::wg_desc_k(sa + L::A_BYTES);
-        br::wg_fence();
+        if constexpr (FP8) {
+            // this thread's A fragments of the unit: 16 bytes per k16 slice (both m64 halves), converted before the first wgmma reads them
+            uint32_t a[BK / 16][2][4];
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-            br::wgmma_ss<BNX>(acc0, br::wg_desc_k(sa) + 2 * k, bdesc + 2 * k, 1);
-            br::wgmma_ss<BNX>(acc1, br::wg_desc_k(sa + 64 * 128) + 2 * k, bdesc + 2 * k, 1);
+            for (int k = 0; k < BK / 16; ++k) {
+                const uint4 q = *reinterpret_cast<const uint4*>(smem + s * L::STAGE + k * 2048 + et * 16);
+                br::fp8w::e4m3x4_to_bf16x2(q.x, a[k][0][0], a[k][1][0]);
+                br::fp8w::e4m3x4_to_bf16x2(q.y, a[k][0][1], a[k][1][1]);
+                br::fp8w::e4m3x4_to_bf16x2(q.z, a[k][0][2], a[k][1][2]);
+                br::fp8w::e4m3x4_to_bf16x2(q.w, a[k][0][3], a[k][1][3]);
+            }
+            br::wg_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) {
+                br::wgmma_rs<BNX>(acc0, a[k][0], bdesc + 2 * k, 1);
+                br::wgmma_rs<BNX>(acc1, a[k][1], bdesc + 2 * k, 1);
+            }
+        } else {
+            br::wg_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) {
+                br::wgmma_ss<BNX>(acc0, br::wg_desc_k(sa) + 2 * k, bdesc + 2 * k, 1);
+                br::wgmma_ss<BNX>(acc1, br::wg_desc_k(sa + 64 * 128) + 2 * k, bdesc + 2 * k, 1);
+            }
         }
         br::wg_commit();
         br::wg_wait<0>();
@@ -183,14 +209,22 @@ __device__ __forceinline__ void compute_row_rstd(const SkParams& p, int et, floa
 }
 
 
+// one weight unit (feature tile `tile`, k block `kb`; unit index u) into a ring stage: a 2-D TMA tile, or the unit's contiguous e4m3 bytes
+template <int BNX, bool FP8>
+__device__ __forceinline__ void load_w(uint8_t* dst, const CUtensorMap* tmW, const SkParams& p, uint64_t* bar, int u, int kb, int tile, uint64_t pol) {
+    if constexpr (FP8) br::bulk_load_hint(dst, p.wq + (long long)u * SL<BNX, FP8>::A_BYTES, SL<BNX, FP8>::A_BYTES, bar, pol);
+    else br::tma_load_2d_hint(dst, tmW, bar, kb * BK, tile * BM, pol);
+}
+
+
 // BNX: wgmma N (rows of X the tensor core sees, zero-filled beyond R); RM: rows the epilogue code is generated for (R <= RM <= BNX).
 // The epilogue runs once per CTA per launch -- straight-line, instruction-fetch-bound code -- so the common R <= 8 decode batch gets its
 // own half-size instantiation.  Warps 0..3: wgmma + epilogue (one feature row per thread), warp 4: TMA producer.
-template <int BNX, int RM>
+template <int BNX, int RM, bool FP8>
 __global__ void __launch_bounds__(NTHREADS, 1)
 skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX,
                   const __grid_constant__ SkParams p) {      // read in place by the helpers (const SkParams&): no register copy
-    using L = SL<BNX>;
+    using L = SL<BNX, FP8>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     float* s_tr = reinterpret_cast<float*>(smem + L::TILE_BYTES);
@@ -223,7 +257,7 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
             for (int i = 0; i < n_pre; ++i) {
                 const int u = u_lo + i, tile = u / p.KB, kb = u - tile * p.KB;
                 br::mbar_expect_tx(&full_bar[i], L::STAGE);
-                br::tma_load_2d_hint(smem + i * L::STAGE, &tmW, &full_bar[i], kb * BK, tile * BM, pol);
+                load_w<BNX, FP8>(smem + i * L::STAGE, &tmW, p, &full_bar[i], u, kb, tile, pol);
             }
             br::grid_dep_wait();
             for (int i = 0; i < n_pre; ++i) {
@@ -236,7 +270,7 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                 br::mbar_wait(&empty_bar[s], ph ^ 1);
                 uint8_t* sa = smem + s * L::STAGE;
                 br::mbar_expect_tx(&full_bar[s], L::STAGE);
-                br::tma_load_2d_hint(sa, &tmW, &full_bar[s], kb * BK, tile * BM, pol);
+                load_w<BNX, FP8>(sa, &tmW, p, &full_bar[s], u, kb, tile, pol);
                 br::tma_load_2d(sa + L::A_BYTES, &tmX, &full_bar[s], kb * BK, 0);
                 if (++s == L::NSTAGE) { s = 0; ph ^= 1; }
             }
@@ -256,8 +290,16 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
             const int part_row = tile * 4 + lane_grp;
             float res[RM];
             load_residual<RM>(p, f, res);                        // in flight while the accumulator is still being produced
+            float wsc = 0.f;
+            if constexpr (FP8) wsc = f < p.N ? __ldcg(p.wscale + f) : 0.f;
             float v[RM];
-            mma_tile<BNX, RM>(smem, full_bar, empty_bar, s, ph, seg_end - u, s_tr, v);
+            mma_tile<BNX, RM, FP8>(smem, full_bar, empty_bar, s, ph, seg_end - u, s_tr, v);
+            if constexpr (FP8) {
+                if (whole) {                                      // the per-row weight scale, once on the finished sum (stream-K: below)
+#pragma unroll
+                    for (int r = 0; r < RM; ++r) v[r] *= wsc;
+                }
+            }
             if (whole) {
                 apply_epilogue<RM>(p, f, lane, v, res, s_rs, part_row);
             } else {
@@ -300,6 +342,10 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
                                 for (int r = 0; r < 8; ++r) v[r0 + r] += t[j][r];            // ascending CTA order: deterministic
                         }
                     }
+                    if constexpr (FP8) {
+#pragma unroll
+                        for (int r = 0; r < RM; ++r) v[r] *= wsc;
+                    }
                     apply_epilogue<RM>(p, f, lane, v, res, s_rs, part_row);
                 }
             }
@@ -308,10 +354,10 @@ skinny_tc5_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
     }
 }
 
-template <int BNX, int RM>
+template <int BNX, int RM, bool FP8>
 int launch(const CUtensorMap& tw, const CUtensorMap& tx, const SkParams& p, int grid, cudaStream_t st) {
-    using L = SL<BNX>;
-    auto kern = skinny_tc5_kernel<BNX, RM>;
+    using L = SL<BNX, FP8>;
+    auto kern = skinny_tc5_kernel<BNX, RM, FP8>;
     static bool done = false;
     if (!done) {
         BR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
@@ -319,6 +365,44 @@ int launch(const CUtensorMap& tw, const CUtensorMap& tx, const SkParams& p, int 
     }
     BR_CHECK_CUDA(br_launch_pdl(kern, dim3(grid), dim3(NTHREADS), (size_t)L::TOTAL, st, tw, tx, p));
     return BR_OK;
+}
+
+// shared host side of br_skinny_gemm / br_skinny_gemm_fp8 (w_scale != NULL: W is the e4m3 buffer of br_quantize_rows_e4m3)
+int skinny_run(const void* X, int64_t ldx, const void* W, int64_t ldw, const float* w_scale, void* out, int64_t ldo, int R, int N, int K,
+               int mode, const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n, float* sumsq_out, float eps,
+               void* stream) {
+    const bool fp8 = w_scale != nullptr;
+    BR_CHECK_ARG(R >= 1 && R <= 32, "skinny_gemm: R=%d must be in [1, 32]", R);
+    BR_CHECK_ARG(N % 16 == 0 && K % 8 == 0 && ldx % 8 == 0 && ldw % 8 == 0, "skinny_gemm: N %% 16, K %% 8, ld %% 8 (N=%d K=%d)", N, K);
+    BR_CHECK_ARG(mode >= 0 && mode <= 3 && !(mode == 1 && !residual), "skinny_gemm: bad mode %d", mode);
+    BR_CHECK_ARG(scratch != nullptr, "skinny_gemm: scratch (br_skinny_scratch_bytes, zero-initialised once) is required");
+    if (fp8) {
+        BR_CHECK_ARG(K % 16 == 0 && ldw == K, "skinny_gemm_fp8: K must be a multiple of 16 and ldw == K (the quantized layout; N=%d K=%d ldw=%lld)",
+                     N, K, (long long)ldw);
+        BR_CHECK_ARG(W != nullptr && ((uintptr_t)W & 15) == 0, "skinny_gemm_fp8: W must be the 16-byte aligned buffer of br_quantize_rows_e4m3");
+    }
+    SkParams p;
+    p.R = R; p.N = N; p.K = K; p.mode = mode; p.out = out; p.ldo = ldo; p.res = (const bf16*)residual; p.ldr = ldr;
+    p.scratch = (float*)scratch; p.counters = (int*)((float*)scratch + (int64_t)br_num_sms() * 32 * BM);
+    p.sumsq_in = sumsq_in; p.sumsq_in_n = sumsq_in_n; p.sumsq_out = sumsq_out; p.eps = eps;
+    p.wq = fp8 ? (const uint8_t*)W : nullptr; p.wscale = w_scale;
+    BR_CHECK_ARG(!(sumsq_out && mode >= 2), "skinny_gemm: sumsq_out only with bf16 outputs (mode 0/1)");
+    p.tiles_n = (N + BM - 1) / BM; p.KB = (K + BK - 1) / BK; p.units = p.tiles_n * p.KB;
+    int grid = p.units < br_num_sms() ? p.units : br_num_sms();
+    p.chunk = (p.units + grid - 1) / grid;
+    grid = (p.units + p.chunk - 1) / p.chunk;
+    const int BNX = R <= 16 ? 16 : 32;
+    CUtensorMap tw, tx;
+    int rc;
+    if ((rc = br_make_tmap_2d_bf16(&tx, X, R, K, ldx, BNX))) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (fp8) {                                                    // the weights come by bulk copy: no weight tensor map
+        if (R <= 8) return launch<16, 8, true>(tx, tx, p, grid, st);
+        return BNX == 16 ? launch<16, 16, true>(tx, tx, p, grid, st) : launch<32, 32, true>(tx, tx, p, grid, st);
+    }
+    if ((rc = br_make_tmap_2d_bf16(&tw, W, N, K, ldw, BM))) return rc;
+    if (R <= 8) return launch<16, 8, false>(tw, tx, p, grid, st);
+    return BNX == 16 ? launch<16, 16, false>(tw, tx, p, grid, st) : launch<32, 32, false>(tw, tx, p, grid, st);
 }
 
 }  // namespace
@@ -333,27 +417,14 @@ int64_t br_skinny_scratch_bytes(int max_N) {
 int br_skinny_gemm(const void* X, int64_t ldx, const void* W, int64_t ldw, void* out, int64_t ldo, int R, int N, int K, int mode,
                    const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n, float* sumsq_out, float eps,
                    void* stream) {
-    BR_CHECK_ARG(R >= 1 && R <= 32, "skinny_gemm: R=%d must be in [1, 32]", R);
-    BR_CHECK_ARG(N % 16 == 0 && K % 8 == 0 && ldx % 8 == 0 && ldw % 8 == 0, "skinny_gemm: N %% 16, K %% 8, ld %% 8 (N=%d K=%d)", N, K);
-    BR_CHECK_ARG(mode >= 0 && mode <= 3 && !(mode == 1 && !residual), "skinny_gemm: bad mode %d", mode);
-    BR_CHECK_ARG(scratch != nullptr, "skinny_gemm: scratch (br_skinny_scratch_bytes, zero-initialised once) is required");
-    SkParams p;
-    p.R = R; p.N = N; p.K = K; p.mode = mode; p.out = out; p.ldo = ldo; p.res = (const bf16*)residual; p.ldr = ldr;
-    p.scratch = (float*)scratch; p.counters = (int*)((float*)scratch + (int64_t)br_num_sms() * 32 * BM);
-    p.sumsq_in = sumsq_in; p.sumsq_in_n = sumsq_in_n; p.sumsq_out = sumsq_out; p.eps = eps;
-    BR_CHECK_ARG(!(sumsq_out && mode >= 2), "skinny_gemm: sumsq_out only with bf16 outputs (mode 0/1)");
-    p.tiles_n = (N + BM - 1) / BM; p.KB = (K + BK - 1) / BK; p.units = p.tiles_n * p.KB;
-    int grid = p.units < br_num_sms() ? p.units : br_num_sms();
-    p.chunk = (p.units + grid - 1) / grid;
-    grid = (p.units + p.chunk - 1) / p.chunk;
-    const int BNX = R <= 16 ? 16 : 32;
-    CUtensorMap tw, tx;
-    int rc;
-    if ((rc = br_make_tmap_2d_bf16(&tw, W, N, K, ldw, BM))) return rc;
-    if ((rc = br_make_tmap_2d_bf16(&tx, X, R, K, ldx, BNX))) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (R <= 8) return launch<16, 8>(tw, tx, p, grid, st);
-    return BNX == 16 ? launch<16, 16>(tw, tx, p, grid, st) : launch<32, 32>(tw, tx, p, grid, st);
+    return skinny_run(X, ldx, W, ldw, nullptr, out, ldo, R, N, K, mode, residual, ldr, scratch, sumsq_in, sumsq_in_n, sumsq_out, eps, stream);
+}
+
+int br_skinny_gemm_fp8(const void* X, int64_t ldx, const void* W, int64_t ldw, const float* w_scale, void* out, int64_t ldo, int R, int N,
+                       int K, int mode, const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n,
+                       float* sumsq_out, float eps, void* stream) {
+    BR_CHECK_ARG(w_scale != nullptr, "skinny_gemm_fp8: w_scale (one fp32 scale per row of W) is required");
+    return skinny_run(X, ldx, W, ldw, w_scale, out, ldo, R, N, K, mode, residual, ldr, scratch, sumsq_in, sumsq_in_n, sumsq_out, eps, stream);
 }
 
 }  // extern "C"

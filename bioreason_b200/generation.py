@@ -125,11 +125,12 @@ class RolloutEngine:
     # ------------------------------------------------------------------
     def rollout_weights(self) -> DecoderW:
         """Merged (base + LoRA) weights with the RMSNorm gains folded in -- decode only; the prefill runs the regular
-        forward (base weights + LoRA second K segment)."""
+        forward (base weights + LoRA second K segment).  With the model's FP8 rollout on, the layer matrices are e4m3 (ops.Fp8Weight)."""
         m = self.model
         if getattr(m, "_rollout_dec", None) is None:
-            from .lora import build_rollout_weights
-            m._rollout_dec = build_rollout_weights(m._dec, m._lora)
+            from .lora import build_rollout_weights, build_rollout_weights_fp8
+            build = build_rollout_weights_fp8 if getattr(m, "_fp8_rollout", False) else build_rollout_weights
+            m._rollout_dec = build(m._dec, m._lora)
         return m._rollout_dec
 
     @torch.no_grad()

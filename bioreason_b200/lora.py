@@ -177,34 +177,74 @@ class LoraState:
         return self.grad_views[idx]
 
 
+# decode matrices whose input is RMS-normed: the norm gain is folded into their columns
+_FOLD = {"w_qkv": "ln1", "w_gu": "ln2"}
+_MATS = ("w_qkv", "w_o", "w_gu", "w_down")
+
+
+def _merge_into(dst, name, Lw, lora, i):
+    """dst <- W + scale * B A of decoder matrix `name` of layer i (W alone without adapters), then the norm gain folded in where
+    the input is normed."""
+    from . import ops
+    base = getattr(Lw, name)
+    if lora is not None:
+        k = name[2:]
+        # [N, K] = B[N, r'] @ (A^T)[K, r']^T ; K-major operands: A_op = B (K = r'), B_op = A^T ([K, r'])
+        ops.gemm(getattr(lora.w.layers[i], "b_" + k), lora.wT[i][f"a_{k}_T"], alpha=lora.scale, residual=base, out=dst)
+    else:
+        dst.copy_(base)
+    if name in _FOLD:
+        ops.scale_columns_(dst, getattr(Lw, _FOLD[name]))
+
+
+def _rollout_shell(dec_w, make):
+    """DecoderW sharing the embedding, with its own final-norm-folded lm_head and per layer the matrices make(Lw, name) returns."""
+    from . import ops
+    from .packing import DecoderLayerW, DecoderW
+    out = DecoderW(cfg=dec_w.cfg, embed=dec_w.embed, lm_head=torch.empty_like(dec_w.lm_head), final_norm=dec_w.final_norm)
+    out.folded = True
+    for Lw in dec_w.layers:
+        out.layers.append(DecoderLayerW(ln1=Lw.ln1, ln2=Lw.ln2, q_norm=Lw.q_norm, k_norm=Lw.k_norm, **{n: make(Lw, n) for n in _MATS}))
+    out.lm_head.copy_(dec_w.lm_head)
+    ops.scale_columns_(out.lm_head, dec_w.final_norm)                      # frozen: folded once
+    return out
+
+
 @torch.no_grad()
 def build_rollout_weights(dec_w, lora: "LoraState | None", out=None):
     """Decode-time weights: W_eff = W + scale * B A per fused weight (the policy that rolls out is base + LoRA; merged with the
     wgmma GEMM, base weight as the epilogue residual), with the RMSNorm gains folded into the columns of the matrices that
     consume a normed input (w_qkv <- ln1, w_gu <- ln2, lm_head <- final norm) so the decode step needs no norm launches."""
-    from . import ops
-    from .packing import DecoderLayerW, DecoderW
     if out is None:
-        out = DecoderW(cfg=dec_w.cfg, embed=dec_w.embed, lm_head=torch.empty_like(dec_w.lm_head), final_norm=dec_w.final_norm)
-        out.folded = True
-        for Lw in dec_w.layers:
-            out.layers.append(DecoderLayerW(ln1=Lw.ln1, ln2=Lw.ln2, q_norm=Lw.q_norm, k_norm=Lw.k_norm, w_qkv=torch.empty_like(Lw.w_qkv),
-                                            w_o=torch.empty_like(Lw.w_o) if lora is not None else Lw.w_o, w_gu=torch.empty_like(Lw.w_gu),
-                                            w_down=torch.empty_like(Lw.w_down) if lora is not None else Lw.w_down))
-        out.lm_head.copy_(dec_w.lm_head)
-        ops.scale_columns_(out.lm_head, dec_w.final_norm)                  # frozen: folded once
+        # without adapters w_o / w_down need neither a merge nor a fold: the frozen base matrices are used as they are
+        out = _rollout_shell(dec_w, lambda Lw, n: torch.empty_like(getattr(Lw, n)) if lora is not None or n in _FOLD else getattr(Lw, n))
     for i, (Lw, Lo) in enumerate(zip(dec_w.layers, out.layers)):
-        if lora is not None:
-            if Lo.w_o.data_ptr() == Lw.w_o.data_ptr() or Lo.w_down.data_ptr() == Lw.w_down.data_ptr():
-                raise RuntimeError("rollout weights alias the frozen base weights (built before enable_lora); rebuild them with out=None")
-            s, Ll, T = lora.scale, lora.w.layers[i], lora.wT[i]
-            # [N, K] = B[N, r'] @ (A^T)[K, r']^T ; K-major operands: A_op = B (K = r'), B_op = A^T ([K, r'])
-            ops.gemm(Ll.b_qkv, T["a_qkv_T"], alpha=s, residual=Lw.w_qkv, out=Lo.w_qkv)
-            ops.gemm(Ll.b_o, T["a_o_T"], alpha=s, residual=Lw.w_o, out=Lo.w_o)
-            ops.gemm(Ll.b_gu, T["a_gu_T"], alpha=s, residual=Lw.w_gu, out=Lo.w_gu)
-            ops.gemm(Ll.b_down, T["a_down_T"], alpha=s, residual=Lw.w_down, out=Lo.w_down)
-        else:
-            Lo.w_qkv.copy_(Lw.w_qkv); Lo.w_gu.copy_(Lw.w_gu)
-        ops.scale_columns_(Lo.w_qkv, Lw.ln1)
-        ops.scale_columns_(Lo.w_gu, Lw.ln2)
+        if lora is not None and (Lo.w_o.data_ptr() == Lw.w_o.data_ptr() or Lo.w_down.data_ptr() == Lw.w_down.data_ptr()):
+            raise RuntimeError("rollout weights alias the frozen base weights (built before enable_lora); rebuild them with out=None")
+        for n in _MATS:
+            if lora is not None or n in _FOLD:
+                _merge_into(getattr(Lo, n), n, Lw, lora, i)
+    return out
+
+
+@torch.no_grad()
+def build_rollout_weights_fp8(dec_w, lora: "LoraState | None", out=None):
+    """The decode weights of build_rollout_weights with the four layer matrices in weight-only FP8 (ops.Fp8Weight: e4m3 codes, one
+    fp32 scale per output row); the embedding and the folded lm_head stay bf16.  Each matrix is merged and folded into one reusable
+    bf16 scratch buffer (the largest matrix) and quantized from there, so no bf16 merged copy of the layers is kept."""
+    from . import ops
+    if out is None:
+        dev = dec_w.embed.device
+        out = _rollout_shell(dec_w, lambda Lw, n: ops.fp8_weight_empty(*getattr(Lw, n).shape, dev))
+        n_max = max(getattr(Lw, n).numel() for Lw in dec_w.layers for n in _MATS)
+        out.fp8_scratch = torch.empty(n_max, device=dev, dtype=torch.bfloat16)
+    for i, (Lw, Lo) in enumerate(zip(dec_w.layers, out.layers)):
+        for n in _MATS:
+            if lora is None and n not in _FOLD:
+                ops.quantize_rows_e4m3(getattr(Lw, n), out=getattr(Lo, n))
+            else:
+                N, K = getattr(Lw, n).shape
+                tmp = out.fp8_scratch[:N * K].view(N, K)
+                _merge_into(tmp, n, Lw, lora, i)
+                ops.quantize_rows_e4m3(tmp, out=getattr(Lo, n))
     return out

@@ -109,6 +109,7 @@ class DNALLMModel(nn.Module):
         self._lora = None
         self._proj_ref = None
         self._rollout_dec = None
+        self._fp8_rollout = False
         self._proj_grad_w = torch.zeros_like(self.dna_projection.weight, dtype=torch.float32)
         self._proj_grad_b = torch.zeros_like(self.dna_projection.bias, dtype=torch.float32)
         self.sync_projection()
@@ -235,6 +236,18 @@ class DNALLMModel(nn.Module):
             raise RuntimeError("set_lora_dropout needs LoRA adapters: call enable_lora first")
         self._lora.set_dropout(p, seed)
 
+    def set_fp8_rollout(self, enabled: bool):
+        """Weight-only FP8 for the rollout decode (off by default): the decode's qkv / o / gate-up / down matrices of every layer are
+        stored as e4m3 with one fp32 scale per output row and streamed at half the bytes; the embedding, the lm_head, the prefill
+        and every training / scoring pass stay bf16.  Rollouts then sample from the quantized policy.  Toggling drops the rollout
+        weights and the decode graphs captured on them; the next rollout rebuilds them in the new format."""
+        enabled = bool(enabled)
+        if enabled != getattr(self, "_fp8_rollout", False):
+            self._fp8_rollout = enabled
+            self._rollout_dec = None
+            if getattr(self, "_rollout", None) is not None:
+                self._rollout._cached.clear()
+
     def new_lora_dropout_pass(self) -> Optional[int]:
         """Pass id shared by the row chunks of one dropout-applying pass (None while dropout is off)."""
         if self._lora is None or self._lora.dropout is None:
@@ -283,8 +296,9 @@ class DNALLMModel(nn.Module):
         if self._lora is not None:
             self._lora.sync()
             if rollout:
-                from ..lora import build_rollout_weights
-                self._rollout_dec = build_rollout_weights(self._dec, self._lora, out=self._rollout_dec)
+                from ..lora import build_rollout_weights, build_rollout_weights_fp8
+                build = build_rollout_weights_fp8 if getattr(self, "_fp8_rollout", False) else build_rollout_weights
+                self._rollout_dec = build(self._dec, self._lora, out=self._rollout_dec)
 
     # ------------------------------------------------------------------ hot path
     def merged_embeddings(self, input_ids, dna_tokenized, batch_idx_map, *, return_proj_inputs: bool = False):

@@ -273,8 +273,37 @@ def skinny_scratch(max_n: int, device) -> torch.Tensor:
     return torch.zeros(lib().br_skinny_scratch_bytes(max_n), device=device, dtype=torch.uint8)
 
 
+class Fp8Weight:
+    """A decode weight [N, K] in weight-only FP8: `q` is br_quantize_rows_e4m3's opaque e4m3 buffer, `scale` the fp32 per-row scales."""
+    __slots__ = ("q", "scale", "shape")
+
+    def __init__(self, q: torch.Tensor, scale: torch.Tensor, shape):
+        self.q, self.scale, self.shape = q, scale, tuple(shape)
+
+
+def fp8_weight_empty(N: int, K: int, device) -> Fp8Weight:
+    q = torch.empty(lib().br_fp8_weight_bytes(N, K), device=device, dtype=torch.uint8)
+    return Fp8Weight(q, torch.empty(N, device=device, dtype=torch.float32), (N, K))
+
+
+def quantize_rows_e4m3(w: torch.Tensor, out: Optional[Fp8Weight] = None) -> Fp8Weight:
+    """Per-row e4m3 quantization of a bf16 [N, K] matrix: scale = amax|row| / 448 (1 for a zero row), codes = RNE(w / scale)."""
+    _need_cuda(w)
+    assert w.dtype == torch.bfloat16 and w.dim() == 2
+    N, K = w.shape
+    if out is None:
+        out = fp8_weight_empty(N, K, w.device)
+    assert out.shape == (N, K)
+    check(lib().br_quantize_rows_e4m3(ptr(w), _row_major_2d(w), N, K, ptr(out.q), ptr(out.scale, "float*"), _stream()), "quantize_rows_e4m3")
+    return out
+
+
 def skinny_gemm(x, w, scratch, *, mode=0, residual=None, out=None, sumsq_in=None, sumsq_in_n=1, sumsq_out=None, eps=0.0):
-    """out[R, N] = x[R, K] @ w[N, K].T for R <= 32 decode rows (optionally with the folded-RMSNorm statistics)."""
+    """out[R, N] = x[R, K] @ w[N, K].T for R <= 32 decode rows (optionally with the folded-RMSNorm statistics).  `w` is a bf16
+    tensor or an Fp8Weight (then w's per-row scales multiply the sums before the epilogue)."""
+    if isinstance(w, Fp8Weight):
+        return _skinny_gemm_fp8(x, w, scratch, mode=mode, residual=residual, out=out, sumsq_in=sumsq_in, sumsq_in_n=sumsq_in_n,
+                                sumsq_out=sumsq_out, eps=eps)
     _need_cuda(x, w)
     R, K = x.shape
     N = w.shape[0]
@@ -288,6 +317,24 @@ def skinny_gemm(x, w, scratch, *, mode=0, residual=None, out=None, sumsq_in=None
                                ptr(sumsq_in, "float*"), int(sumsq_in_n) if sumsq_in is not None else 0, ptr(sumsq_out, "float*"),
                                float(eps), _stream()),
           "skinny_gemm")
+    return out
+
+
+def _skinny_gemm_fp8(x, w, scratch, *, mode, residual, out, sumsq_in, sumsq_in_n, sumsq_out, eps):
+    _need_cuda(x, w.q)
+    R, K = x.shape
+    N = w.shape[0]
+    assert w.shape[1] == K, (w.shape, x.shape)
+    if out is None:
+        if mode == 3:
+            out = torch.empty(R, N, device=x.device, dtype=torch.float32)
+        else:
+            out = torch.empty(R, N // 2 if mode == 2 else N, device=x.device, dtype=torch.bfloat16)
+    check(lib().br_skinny_gemm_fp8(ptr(x), _row_major_2d(x), ptr(w.q), K, ptr(w.scale, "float*"), ptr(out), _row_major_2d(out), R, N, K, mode,
+                                   ptr(residual), _row_major_2d(residual) if residual is not None else 0, ptr(scratch),
+                                   ptr(sumsq_in, "float*"), int(sumsq_in_n) if sumsq_in is not None else 0, ptr(sumsq_out, "float*"),
+                                   float(eps), _stream()),
+          "skinny_gemm_fp8")
     return out
 
 

@@ -73,3 +73,4 @@ class DNALLMGRPOConfig:
     micro_rows: Optional[int] = None      # rows per forward/backward chunk (None = as many as the device memory holds)
     suppress_eos: bool = False            # fixed-length rollouts (bench config c)
     share_prompt_prefix: bool = False     # ref / old / policy passes compute each prompt group's full prompt tiles once (same log-probs)
+    fp8_rollout: bool = False             # rollout decode streams e4m3 layer weights (per-row scales); samples from the quantized policy

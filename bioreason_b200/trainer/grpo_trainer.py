@@ -115,6 +115,8 @@ class DNALLMGRPOTrainer:
                              "of a prompt, so the prompt cannot be computed once")
         if model._lora is None:
             model.enable_lora(r=a.lora_r, alpha=a.lora_alpha, seed=a.seed)
+        # each rank quantizes its own (identical) merged weights; the quantizer is deterministic, so the ranks agree
+        model.set_fp8_rollout(getattr(a, "fp8_rollout", False))
         model.sync_adapters(rollout=True)
         if a.apply_lora_dropout:                                            # peft's rate; per-rank masks (set_seed(device_specific=True))
             p = getattr(model, "lora_dropout", None)

@@ -164,6 +164,17 @@ int64_t br_skinny_scratch_bytes(int max_N);
 int br_skinny_gemm(const void* X, int64_t ldx, const void* W, int64_t ldw, void* out, int64_t ldo, int R, int N, int K, int mode,
                    const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n, float* sumsq_out,
                    float eps, void* stream);
+/* Weight-only FP8 (e4m3) for the rollout decode.  br_quantize_rows_e4m3: W [N, K] bf16 (row stride ldw, K % 16 == 0) ->
+ * scale [N] fp32 = amax_k |W[n, k]| / 448 (1 for an all-zero row) and Q = e4m3fn(W[n, k] / scale[n]) (round to nearest even, never a
+ * NaN code) in a private layout of br_fp8_weight_bytes(N, K) bytes (16-byte aligned) that only br_skinny_gemm_fp8 reads.
+ * br_skinny_gemm_fp8: br_skinny_gemm with W = that buffer (ldw = K) and out[r, n] = scale[n] * (X . dequantized-codes^T)[r, n]
+ * before the mode's epilogue (mode 2: gate and up features each with their own scale); same modes, statistics, scratch and
+ * reproducibility. */
+int64_t br_fp8_weight_bytes(int N, int K);
+int br_quantize_rows_e4m3(const void* W, int64_t ldw, int N, int K, void* Q, float* scale, void* stream);
+int br_skinny_gemm_fp8(const void* X, int64_t ldx, const void* W, int64_t ldw, const float* w_scale, void* out, int64_t ldo, int R, int N,
+                       int K, int mode, const void* residual, int64_t ldr, void* scratch, const float* sumsq_in, int sumsq_in_n,
+                       float* sumsq_out, float eps, void* stream);
 int br_embed_gather_sumsq(const int64_t* ids, const void* table, int64_t ldt, int64_t vocab, void* out, int64_t ldo, int M, int d,
                           float* sumsq, void* stream);
 /* W[n, k] *= scale[k] in place (bf16) */
