@@ -38,14 +38,21 @@ __global__ void advantages_kernel(const float* __restrict__ rpf, int rows, int n
     }
 }
 
-// one CTA, one warp per row (strided); fixed-order reductions -> deterministic
+// one CTA, one warp per row (strided); fixed-order reductions -> deterministic.
+// IS: truncated importance sampling against the rollout's own log-probs b = rollout_lp: the policy-gradient term of each token is
+// weighted by w = min(exp(o - b), is_cap) with o = old_lp (lp when old_lp is NULL), a value without gradient; the KL term is not
+// weighted.  is_stats = masked token means of {w, [exp(o - b) > is_cap], o - b, exp(o - b) - 1 - (o - b)}.
+template <bool IS>
 __global__ void __launch_bounds__(1024) grpo_loss_kernel(const float* __restrict__ lp, const float* __restrict__ old_lp,
                                                          const float* __restrict__ ref_lp, const float* __restrict__ adv,
                                                          const int* __restrict__ mask, int B, int C, float beta, float eps_lo,
-                                                         float eps_hi, float* __restrict__ out3, float* __restrict__ dlp) {
+                                                         float eps_hi, float* __restrict__ out3, float* __restrict__ dlp,
+                                                         const float* __restrict__ rollout_lp, float is_cap, float* __restrict__ is_stats) {
     __shared__ float s_loss[32], s_kl[32], s_clip[32], s_cnt[32];
+    __shared__ float s_is[IS ? 4 : 1][32];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
     float w_loss = 0.f, w_kl = 0.f, w_clip = 0.f, w_cnt = 0.f;
+    float w_is[4] = {0.f, 0.f, 0.f, 0.f};
     for (int b = warp; b < B; b += nwarps) {
         float cnt = 0.f;
         for (int t = lane; t < C; t += 32) cnt += (float)mask[(size_t)b * C + t];
@@ -53,6 +60,7 @@ __global__ void __launch_bounds__(1024) grpo_loss_kernel(const float* __restrict
         const float a = adv[b];
         const float inv = cnt > 0.f ? 1.f / (cnt * (float)B) : 0.f;
         float rl = 0.f, rk = 0.f, rc = 0.f;
+        float ris[4] = {0.f, 0.f, 0.f, 0.f};
         for (int t = lane; t < C; t += 32) {
             const size_t i = (size_t)b * C + t;
             const float x = lp[i];
@@ -65,6 +73,14 @@ __global__ void __launch_bounds__(1024) grpo_loss_kernel(const float* __restrict
             if (l1 < l2) g = -c1 * a;
             else if (l1 > l2) g = (c1 > 1.f - eps_lo && c1 < 1.f + eps_hi) ? -c1 * a : 0.f;
             else g = (c1 >= 1.f - eps_lo && c1 <= 1.f + eps_hi) ? -c1 * a : -0.5f * c1 * a;
+            if constexpr (IS) {
+                const float d = o - rollout_lp[i];
+                const float r = expf(d);
+                const float w = fminf(r, is_cap);
+                l *= w; g *= w;
+                const float m = (float)mask[i];
+                ris[0] += w * m; ris[1] += (r > is_cap ? m : 0.f); ris[2] += d * m; ris[3] += (r - 1.f - d) * m;
+            }
             float kl = 0.f;
             if (beta > 0.f && ref_lp) {
                 const float d = ref_lp[i] - x;
@@ -80,14 +96,31 @@ __global__ void __launch_bounds__(1024) grpo_loss_kernel(const float* __restrict
         rl = br::warp_sum(rl); rk = br::warp_sum(rk); rc = br::warp_sum(rc);
         if (cnt > 0.f) { w_loss += rl / cnt; w_kl += rk / cnt; }
         w_clip += rc; w_cnt += cnt;
+        if constexpr (IS) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) w_is[j] += br::warp_sum(ris[j]);
+        }
     }
     if (lane == 0) { s_loss[warp] = w_loss; s_kl[warp] = w_kl; s_clip[warp] = w_clip; s_cnt[warp] = w_cnt; }
+    if constexpr (IS) {
+        if (lane == 0) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) s_is[j][warp] = w_is[j];
+        }
+    }
     __syncthreads();
     if (warp == 0) {
         float a = lane < nwarps ? s_loss[lane] : 0.f, k = lane < nwarps ? s_kl[lane] : 0.f;
         float c = lane < nwarps ? s_clip[lane] : 0.f, n = lane < nwarps ? s_cnt[lane] : 0.f;
         a = br::warp_sum(a); k = br::warp_sum(k); c = br::warp_sum(c); n = br::warp_sum(n);
         if (lane == 0) { out3[0] = a / (float)B; out3[1] = k / (float)B; out3[2] = n > 0.f ? c / n : 0.f; }
+        if constexpr (IS) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const float s = br::warp_sum(lane < nwarps ? s_is[j][lane] : 0.f);
+                if (lane == 0) is_stats[j] = n > 0.f ? s / n : 0.f;
+            }
+        }
     }
 }
 
@@ -120,7 +153,22 @@ int br_grpo_loss_fwd_bwd(const float* lp, const float* old_lp, const float* ref_
     BR_CHECK_ARG(B > 0 && C > 0, "grpo_loss: empty batch");
     BR_CHECK_ARG(!(beta > 0.f && !ref_lp), "grpo_loss: beta > 0 needs ref_lp");
     int threads = B >= 32 ? 1024 : B * 32;
-    grpo_loss_kernel<<<1, threads, 0, (cudaStream_t)stream>>>(lp, old_lp, ref_lp, adv, mask, B, C, beta, eps_low, eps_high, out3, dlp);
+    grpo_loss_kernel<false><<<1, threads, 0, (cudaStream_t)stream>>>(lp, old_lp, ref_lp, adv, mask, B, C, beta, eps_low, eps_high, out3, dlp,
+                                                                     nullptr, 0.f, nullptr);
+    BR_CHECK_LAUNCH();
+    return BR_OK;
+}
+
+int br_grpo_loss_is_fwd_bwd(const float* lp, const float* old_lp, const float* ref_lp, const float* rollout_lp, const float* adv,
+                            const int32_t* mask, int B, int C, float beta, float eps_low, float eps_high, float is_cap, float* out3,
+                            float* is_stats, float* dlp, void* stream) {
+    BR_CHECK_ARG(B > 0 && C > 0, "grpo_loss_is: empty batch");
+    BR_CHECK_ARG(!(beta > 0.f && !ref_lp), "grpo_loss_is: beta > 0 needs ref_lp");
+    BR_CHECK_ARG(rollout_lp && is_stats, "grpo_loss_is: needs rollout_lp and is_stats");
+    BR_CHECK_ARG(is_cap > 0.f, "grpo_loss_is: is_cap must be > 0 (+inf: untruncated), got %g", (double)is_cap);
+    int threads = B >= 32 ? 1024 : B * 32;
+    grpo_loss_kernel<true><<<1, threads, 0, (cudaStream_t)stream>>>(lp, old_lp, ref_lp, adv, mask, B, C, beta, eps_low, eps_high, out3, dlp,
+                                                                    rollout_lp, is_cap, is_stats);
     BR_CHECK_LAUNCH();
     return BR_OK;
 }

@@ -92,6 +92,21 @@ __device__ __forceinline__ float block_max(float v, float* s_red) {   // all thr
     __syncthreads();
     return m;
 }
+// fixed-order block sum: thread 0 gets the total (the same bits on every call); s_red: 32 floats
+__device__ __forceinline__ float block_sum(float v, float* s_red) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
+    v = br::warp_sum(v);
+    if (lane == 0) s_red[warp] = v;
+    __syncthreads();
+    float s = lane < nw ? s_red[lane] : 0.f;
+    s = br::warp_sum(s);
+    __syncthreads();
+    return s;
+}
+
+// Behaviour log-prob (the *_logp entry points): logp[r, step] = z[y] - logsumexp(z) over the raw fp32 logits of the row (T = 1, the
+// full vocabulary) -- the quantity br_lmhead_logprob_fwd gives the scoring passes.  Two-stage path: stage 1 writes each chunk's
+// (max m_c, sum exp(z - m_c)), stage 2 combines the pairs in chunk order; single stage: a block-wide LSE over the row.
 
 // Stage 1 (many CTAs): each CTA owns a 4096-logit chunk of one row, keeps it in registers, finds the chunk's exact
 // top_k-th value by radix select on shared-memory histograms and emits every element >= that value (value, token id) --
@@ -99,8 +114,10 @@ __device__ __forceinline__ float block_max(float v, float* s_red) {   // all thr
 // candidates instead of 151 936 logits: the sampler drops from ~200 us to ~20 us per decode step.
 constexpr int CHUNK = 4096, CAND_CAP = 64;
 
+template <bool LOGP>
 __global__ void __launch_bounds__(256) sampler_partial_kernel(const float* __restrict__ logits, long long ld, int V, int top_k,
-                                                              float* __restrict__ cand_val, int* __restrict__ cand_idx, int n_chunks) {
+                                                              float* __restrict__ cand_val, int* __restrict__ cand_idx, int n_chunks,
+                                                              float2* __restrict__ chunk_stats) {
     __shared__ int hist[2048];
     __shared__ int s_tmp[4];
     __shared__ int s_count;
@@ -130,6 +147,17 @@ __global__ void __launch_bounds__(256) sampler_partial_kernel(const float* __res
 #pragma unroll
         for (int i = 0; i < 16; ++i) mx = fmaxf(mx, v[i]);
         mx = block_max(mx, s_red);
+        if constexpr (LOGP) {
+            // (m_c, s_c) before the fast / exact split (the fast path returns early); entries past V hold -inf and add 0, and an
+            // all -inf chunk gives (-inf, 0)
+            float s = 0.f;
+            if (mx > -INFINITY) {
+#pragma unroll
+                for (int i = 0; i < 16; ++i) s += expf(v[i] - mx);
+            }
+            s = block_sum(s, s_red);
+            if (tid == 0) chunk_stats[(long long)row * n_chunks + chunk] = make_float2(mx, s);
+        }
         for (int i = tid; i < FBINS; i += 256) hist[i] = 0;
         if (tid == 0) s_count = 0;
         __syncthreads();
@@ -219,11 +247,14 @@ __global__ void __launch_bounds__(256) sampler_partial_kernel(const float* __res
 }
 
 // Stage 2 / single-stage sampler.  cand_idx == nullptr: x is the full logits row (index = position).
+// LOGP: also writes logp[row, step]; chunk_stats = stage 1's n_chunks (m_c, s_c) pairs per row, or nullptr (single stage: x is the row).
+template <bool LOGP>
 __global__ void __launch_bounds__(1024) sampler_kernel(const float* __restrict__ logits, long long ld, int V, const int* __restrict__ cand_idx_all, float temperature, int top_k,
                                                        float top_p, int do_sample, const float* __restrict__ uniforms,
                                                        const int* __restrict__ step_ptr, int R, int max_steps, long long eos_id,
                                                        long long pad_id, int* __restrict__ finished, long long* __restrict__ tokens,
-                                                       long long* __restrict__ next_ids) {
+                                                       long long* __restrict__ next_ids, const float2* __restrict__ chunk_stats, int n_chunks,
+                                                       float* __restrict__ logp) {
     __shared__ int hist[2048];
     __shared__ int s_tmp[4];
     __shared__ float c_val[MAXC];
@@ -233,6 +264,7 @@ __global__ void __launch_bounds__(1024) sampler_kernel(const float* __restrict__
     __shared__ int s_count;
     __shared__ float r_val[32];
     __shared__ int r_idx[32];
+    __shared__ float s_chosen_z;                                       // LOGP: the chosen token's raw logit
 
     const int row = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     br::launch_dependents();
@@ -261,6 +293,7 @@ __global__ void __launch_bounds__(1024) sampler_kernel(const float* __restrict__
                 if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
             }
             if (lane == 0) s_tmp[2] = bi;
+            if constexpr (LOGP) { if (lane == 0) s_chosen_z = bv; }
         }
         __syncthreads();
         choice = s_tmp[2];
@@ -374,21 +407,47 @@ __global__ void __launch_bounds__(1024) sampler_kernel(const float* __restrict__
             const float target = u * ktot;
             // selection by repeatedly taking the smallest remaining id (keep is ~20)
             float acc = 0.f; int chosen = o_idx[0]; int last_id = -1;
+            float chosen_z = o_val[0];
             for (int n = 0; n < keep; ++n) {
                 int best = -1;
                 for (int j = 0; j < keep; ++j) if (o_idx[j] > last_id && (best < 0 || o_idx[j] < o_idx[best])) best = j;
                 acc += c_val[best]; last_id = o_idx[best]; chosen = o_idx[best];
+                if constexpr (LOGP) chosen_z = o_val[best];
                 if (acc > target) break;
             }
             s_tmp[2] = chosen;
+            if constexpr (LOGP) s_chosen_z = chosen_z;
         }
         __syncthreads();
         choice = s_tmp[2];
+    }
+    float lse = 0.f;                                                   // valid in thread 0
+    if constexpr (LOGP) {
+        if (chunk_stats) {
+            if (warp == 0) {
+                const float2* st = chunk_stats + (long long)row * n_chunks;
+                float m = -INFINITY;
+                for (int c = lane; c < n_chunks; c += 32) m = fmaxf(m, __ldcg(&st[c].x));
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+                float s = 0.f;
+                for (int c = lane; c < n_chunks; c += 32) { const float2 p = __ldcg(st + c); s += p.y * expf(p.x - m); }
+                lse = m + logf(br::warp_sum(s));
+            }
+        } else {
+            float m = -INFINITY;
+            for (int i = tid; i < V; i += blockDim.x) m = fmaxf(m, __ldcg(x + i));
+            m = block_max(m, r_val);
+            float s = 0.f;
+            if (m > -INFINITY) for (int i = tid; i < V; i += blockDim.x) s += expf(__ldcg(x + i) - m);
+            lse = m + logf(block_sum(s, r_val));
+        }
     }
     if (tid == 0) {
         const int fin = finished ? __ldcg(finished + row) : 0;
         long long tok = fin ? pad_id : choice;                         // finished rows emit pad (HF :2796-2797)
         if (tokens && step < max_steps) tokens[(long long)row * max_steps + step] = tok;
+        if constexpr (LOGP) { if (step < max_steps) logp[(long long)row * max_steps + step] = fin ? 0.f : s_chosen_z - lse; }
         if (next_ids) next_ids[row] = tok;
         if (finished && !fin && eos_id >= 0 && tok == eos_id) finished[row] = 1;
     }
@@ -415,8 +474,23 @@ int br_sample_next(const float* logits, int64_t ld, int R, int V, float temperat
     if (do_sample) {
         BR_CHECK_ARG(temperature > 0.f && top_k >= 1 && top_k <= MAXC && top_p > 0.f && uniforms, "sample_next: need T > 0, 1 <= top_k <= %d, top_p > 0 and a uniforms buffer", MAXC);
     }
-    sampler_kernel<<<R, 1024, 0, (cudaStream_t)stream>>>(logits, ld, V, nullptr, temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps,
-                                                        (long long)eos_id, (long long)pad_id, finished, (long long*)tokens, (long long*)next_ids);
+    sampler_kernel<false><<<R, 1024, 0, (cudaStream_t)stream>>>(logits, ld, V, nullptr, temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps,
+                                                               (long long)eos_id, (long long)pad_id, finished, (long long*)tokens, (long long*)next_ids,
+                                                               nullptr, 0, nullptr);
+    BR_CHECK_LAUNCH();
+    return BR_OK;
+}
+
+int br_sample_next_logp(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
+                        const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id, int32_t* finished,
+                        int64_t* tokens, int64_t* next_ids, float* logp, void* stream) {
+    BR_CHECK_ARG(R > 0 && V > 0 && logp, "sample_next_logp: empty / no logp buffer");
+    if (do_sample) {
+        BR_CHECK_ARG(temperature > 0.f && top_k >= 1 && top_k <= MAXC && top_p > 0.f && uniforms, "sample_next_logp: need T > 0, 1 <= top_k <= %d, top_p > 0 and a uniforms buffer", MAXC);
+    }
+    sampler_kernel<true><<<R, 1024, 0, (cudaStream_t)stream>>>(logits, ld, V, nullptr, temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps,
+                                                              (long long)eos_id, (long long)pad_id, finished, (long long*)tokens, (long long*)next_ids,
+                                                              nullptr, 0, logp);
     BR_CHECK_LAUNCH();
     return BR_OK;
 }
@@ -426,10 +500,14 @@ int64_t br_sample_workspace_bytes(int R, int V) {
     return (int64_t)R * n_chunks * CAND_CAP * (sizeof(float) + sizeof(int));
 }
 
-/* two-stage variant for large vocabularies (same semantics as br_sample_next) */
-int br_sample_next_2stage(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
-                          const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id, int32_t* finished,
-                          int64_t* tokens, int64_t* next_ids, void* workspace, void* stream) {
+int64_t br_sample_logp_workspace_bytes(int R, int V) {
+    const int n_chunks = (V + CHUNK - 1) / CHUNK;
+    return br_sample_workspace_bytes(R, V) + (int64_t)R * n_chunks * sizeof(float2);
+}
+
+static int sample_2stage(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
+                         const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id, int32_t* finished,
+                         int64_t* tokens, int64_t* next_ids, float* logp, void* workspace, void* stream) {
     BR_CHECK_ARG(R > 0 && V > 0 && workspace, "sample_next_2stage: empty / no workspace");
     const int k = do_sample ? top_k : 1;
     BR_CHECK_ARG(k >= 1 && k <= CAND_CAP / 2, "sample_next_2stage: top_k must be in [1, %d]", CAND_CAP / 2);
@@ -438,12 +516,37 @@ int br_sample_next_2stage(const float* logits, int64_t ld, int R, int V, float t
     float* cv = (float*)workspace;
     int* ci = (int*)(cv + (int64_t)R * n_chunks * CAND_CAP);
     cudaStream_t st = (cudaStream_t)stream;
-    BR_CHECK_CUDA(br_launch_pdl(sampler_partial_kernel, dim3(n_chunks, R), dim3(256), 0, st, logits, (long long)ld, V, k, cv, ci, n_chunks));
     const int n_cand = n_chunks * CAND_CAP;
-    BR_CHECK_CUDA(br_launch_pdl(sampler_kernel, dim3(R), dim3(1024), 0, st, (const float*)cv, (long long)n_cand, n_cand, (const int*)ci, temperature,
-                                top_k, top_p, do_sample, uniforms, step, R, max_steps, (long long)eos_id, (long long)pad_id, finished,
-                                (long long*)tokens, (long long*)next_ids));
+    if (!logp) {
+        BR_CHECK_CUDA(br_launch_pdl(sampler_partial_kernel<false>, dim3(n_chunks, R), dim3(256), 0, st, logits, (long long)ld, V, k, cv, ci, n_chunks,
+                                    (float2*)nullptr));
+        BR_CHECK_CUDA(br_launch_pdl(sampler_kernel<false>, dim3(R), dim3(1024), 0, st, (const float*)cv, (long long)n_cand, n_cand, (const int*)ci,
+                                    temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps, (long long)eos_id, (long long)pad_id,
+                                    finished, (long long*)tokens, (long long*)next_ids, (const float2*)nullptr, 0, (float*)nullptr));
+        return BR_OK;
+    }
+    float2* stats = (float2*)(ci + (int64_t)R * n_chunks * CAND_CAP);       // the tail of br_sample_logp_workspace_bytes
+    BR_CHECK_CUDA(br_launch_pdl(sampler_partial_kernel<true>, dim3(n_chunks, R), dim3(256), 0, st, logits, (long long)ld, V, k, cv, ci, n_chunks, stats));
+    BR_CHECK_CUDA(br_launch_pdl(sampler_kernel<true>, dim3(R), dim3(1024), 0, st, (const float*)cv, (long long)n_cand, n_cand, (const int*)ci,
+                                temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps, (long long)eos_id, (long long)pad_id,
+                                finished, (long long*)tokens, (long long*)next_ids, (const float2*)stats, n_chunks, logp));
     return BR_OK;
+}
+
+/* two-stage variant for large vocabularies (same semantics as br_sample_next) */
+int br_sample_next_2stage(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
+                          const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id, int32_t* finished,
+                          int64_t* tokens, int64_t* next_ids, void* workspace, void* stream) {
+    return sample_2stage(logits, ld, R, V, temperature, top_k, top_p, do_sample, uniforms, step, max_steps, eos_id, pad_id, finished, tokens,
+                         next_ids, nullptr, workspace, stream);
+}
+
+int br_sample_next_2stage_logp(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
+                               const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id, int32_t* finished,
+                               int64_t* tokens, int64_t* next_ids, float* logp, void* workspace, void* stream) {
+    BR_CHECK_ARG(logp, "sample_next_2stage_logp: no logp buffer");
+    return sample_2stage(logits, ld, R, V, temperature, top_k, top_p, do_sample, uniforms, step, max_steps, eos_id, pad_id, finished, tokens,
+                         next_ids, logp, workspace, stream);
 }
 
 int br_decode_advance(int32_t* step, int32_t* cur_len, int R, void* stream) {

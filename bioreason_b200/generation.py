@@ -135,7 +135,10 @@ class RolloutEngine:
 
     @torch.no_grad()
     def generate(self, input_ids, attention_mask, dna_tokenized=None, batch_idx_map=None, *, params: SamplingParams,
-                 uniforms: Optional[torch.Tensor] = None, use_graph: bool = True, return_stats: bool = False):
+                 uniforms: Optional[torch.Tensor] = None, use_graph: bool = True, return_stats: bool = False,
+                 return_logprobs: bool = False):
+        """Completion ids [B, <= C]; return_logprobs: also the fp32 log-prob of each sampled token under the decode's own raw logits
+        (T = 1, full vocabulary; 0 after a row's EOS), trimmed like the ids -- the behaviour log-probs of the rollout."""
         m = self.model
         W = m._dec                                                          # prefill weights
         Wd = self.rollout_weights()                                         # decode weights (merged + folded)
@@ -186,7 +189,7 @@ class RolloutEngine:
         # Static buffers + the captured decode graph are cached per rollout shape: a training run replays the same graph every
         # step (no per-step capture, no graph-pool / allocator churn -- that churn showed up as multi-second host stalls).
         key = (B, G, tuple(plen), C, n_shared, max_pages, n_pages, params.do_sample, params.temperature, params.top_k, params.top_p,
-               params.eos_token_id, params.pad_token_id, id(Wd), bool(use_graph))
+               params.eos_token_id, params.pad_token_id, id(Wd), bool(use_graph), bool(return_logprobs))
         St = self._cached.get(key)
         hit = St is not None
         if not hit:
@@ -225,6 +228,7 @@ class RolloutEngine:
         cur0 = torch.tensor([plen[r // G] for r in range(R)], device=dev, dtype=torch.int32)
         if not hit:
             St.tokens = torch.full((R, C), pad_fill, device=dev, dtype=torch.int64)
+            St.logp = torch.zeros(R, C, device=dev, dtype=torch.float32) if return_logprobs else None
             St.next_ids = torch.zeros(R, device=dev, dtype=torch.int64)
             St.finished = torch.zeros(R, device=dev, dtype=torch.int32)
             St.step = torch.zeros(1, device=dev, dtype=torch.int32)
@@ -254,13 +258,16 @@ class RolloutEngine:
             St.ssq_a = torch.zeros(n_part_, 32, device=dev, dtype=torch.float32)    # sum x^2 of the residual stream entering attention
             St.ssq_b = torch.zeros(n_part_, 32, device=dev, dtype=torch.float32)    # ... entering the MLP (see br_skinny_gemm)
             St.ssq_e = torch.zeros(1, 32, device=dev, dtype=torch.float32)          # ... of the embedding row (first layer)
-            St.samp_ws = ops.sample_workspace(R, cfg.vocab_size, dev)
+            St.samp_ws = ops.sample_workspace(R, cfg.vocab_size, dev, logp=return_logprobs)
             St.graph = None
         else:
             St.tokens.fill_(pad_fill); St.finished.zero_(); St.step.zero_(); St.cur_len.copy_(cur0)
+            if return_logprobs:
+                St.logp.zero_()
             if params.do_sample:
                 St.uniforms.copy_(uniforms)
         tokens, next_ids, finished, step, cur_len = St.tokens, St.next_ids, St.finished, St.step, St.cur_len
+        logp_kw = dict(logp=St.logp) if return_logprobs else {}
         uniforms = St.uniforms
         scratch, ws, attn_out, rope, h = St.scratch, St.ws, St.attn_out, St.rope, St.h
         ssq_a, ssq_b, ssq_e, samp_ws = St.ssq_a, St.ssq_b, St.ssq_e, St.samp_ws
@@ -271,7 +278,7 @@ class RolloutEngine:
             ops.sample_next(logits, workspace=samp_ws, temperature=params.temperature, top_k=params.top_k, top_p=params.top_p, do_sample=params.do_sample,
                             uniforms=uniforms if params.do_sample else None, step=step, max_steps=C, eos_id=eos,
                             pad_id=params.pad_token_id if params.pad_token_id is not None else 0, finished=finished, tokens=tokens,
-                            next_ids=next_ids)
+                            next_ids=next_ids, **logp_kw)
 
         # ---- first token from the prefill's last position (row u replicated G times)
         last_rows = torch.tensor([u * P + P - 1 for u in range(U) for _ in range(G)], device=dev, dtype=torch.int32)
@@ -355,6 +362,7 @@ class RolloutEngine:
             is_eos = out == eos
             first = torch.where(is_eos.any(1), is_eos.int().argmax(1) + 1, torch.full((R,), min(done_steps + 1, C), device=dev))
             out = out[:, : int(first.max().item())]
+        res = (out, St.logp[:, : out.shape[1]].clone()) if return_logprobs else (out,)
         if return_stats:
-            return out, dict(G=G, unique_prompts=U, n_shared_pages=n_shared, pages=n_pages, graph=graph is not None)
-        return out
+            res += (dict(G=G, unique_prompts=U, n_shared_pages=n_shared, pages=n_pages, graph=graph is not None),)
+        return res if len(res) > 1 else out

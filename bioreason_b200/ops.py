@@ -55,6 +55,28 @@ def grpo_loss_raw(lp, old_lp, ref_lp, adv, mask, beta, eps_low, eps_high, want_g
     return out3, dlp
 
 
+def grpo_loss_is_raw(lp, old_lp, ref_lp, rollout_lp, adv, mask, beta, eps_low, eps_high, is_cap, want_grad=True):
+    """grpo_loss_raw with truncated importance sampling against the rollout's log-probs (br_grpo_loss_is_fwd_bwd): each token's
+    policy-gradient term is weighted by min(exp(o - rollout_lp), is_cap), o = old_lp (lp when None), the KL term is not.
+    Returns (out3, is_stats, dlp); is_stats = masked token means of [w, capped, o - rollout_lp, exp(o - rollout_lp) - 1 - (o - rollout_lp)]."""
+    _need_cuda(lp, rollout_lp, adv, mask)
+    B, C = lp.shape
+    lp = lp.float().contiguous()
+    old_lp = None if old_lp is None else old_lp.float().contiguous()
+    ref_lp = None if ref_lp is None else ref_lp.float().contiguous()
+    rollout_lp = rollout_lp.float().contiguous()
+    assert rollout_lp.shape == (B, C), (rollout_lp.shape, lp.shape)
+    adv = adv.float().contiguous()
+    mask = mask.to(torch.int32).contiguous()
+    out3 = torch.empty(3, device=lp.device, dtype=torch.float32)
+    stats = torch.empty(4, device=lp.device, dtype=torch.float32)
+    dlp = torch.empty_like(lp) if want_grad else None
+    check(lib().br_grpo_loss_is_fwd_bwd(ptr(lp, "float*"), ptr(old_lp, "float*"), ptr(ref_lp, "float*"), ptr(rollout_lp, "float*"),
+                                        ptr(adv, "float*"), ptr(mask, "int32_t*"), B, C, float(beta), float(eps_low), float(eps_high),
+                                        float(is_cap), ptr(out3, "float*"), ptr(stats, "float*"), ptr(dlp, "float*"), _stream()), "grpo_loss_is")
+    return out3, stats, dlp
+
+
 class _GRPOLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, lp, old_lp, ref_lp, adv, mask, beta, eps_low, eps_high):
@@ -379,14 +401,21 @@ def decode_attn_fused(qkv_raw, q_norm_w, k_norm_w, kcache, vcache, page_table, c
     return out
 
 
-def sample_workspace(R, V, device):
-    return torch.empty(lib().br_sample_workspace_bytes(R, V), device=device, dtype=torch.uint8)
+def sample_workspace(R, V, device, logp: bool = False):
+    """Two-stage sampler workspace; logp=True: large enough for sample_next(..., logp=) as well."""
+    n = lib().br_sample_logp_workspace_bytes(R, V) if logp else lib().br_sample_workspace_bytes(R, V)
+    return torch.empty(n, device=device, dtype=torch.uint8)
 
 
 def sample_next(logits, *, temperature=1.0, top_k=20, top_p=1.0, do_sample=True, uniforms=None, step=None, max_steps=1,
-                eos_id=-1, pad_id=0, finished=None, tokens=None, next_ids=None, workspace=None):
+                eos_id=-1, pad_id=0, finished=None, tokens=None, next_ids=None, workspace=None, logp=None):
+    """logp: optional fp32 [R, max_steps]; receives log_softmax(logits)[r, token] at column step (0 for finished rows)."""
     R, V = logits.shape
     assert logits.dtype == torch.float32
+    if logp is not None:
+        _sample_next_logp(logits, R, V, temperature, top_k, top_p, do_sample, uniforms, step, max_steps, eos_id, pad_id, finished, tokens,
+                          next_ids, workspace, logp)
+        return
     if workspace is not None and (not do_sample or top_k <= 32):
         check(lib().br_sample_next_2stage(ptr(logits, "float*"), _row_major_2d(logits), R, V, float(temperature), int(top_k), float(top_p),
                                           1 if do_sample else 0, ptr(uniforms, "float*"), ptr(step, "int32_t*"), int(max_steps), int(eos_id),
@@ -397,6 +426,23 @@ def sample_next(logits, *, temperature=1.0, top_k=20, top_p=1.0, do_sample=True,
                                1 if do_sample else 0, ptr(uniforms, "float*"), ptr(step, "int32_t*"), int(max_steps), int(eos_id),
                                int(pad_id), ptr(finished, "int32_t*"), ptr(tokens, "int64_t*"), ptr(next_ids, "int64_t*"), _stream()),
           "sample_next")
+
+
+def _sample_next_logp(logits, R, V, temperature, top_k, top_p, do_sample, uniforms, step, max_steps, eos_id, pad_id, finished, tokens,
+                      next_ids, workspace, logp):
+    _need_cuda(logits, logp)
+    assert logp.dtype == torch.float32 and logp.is_contiguous() and logp.shape == (R, max_steps), (logp.shape, R, max_steps)
+    if workspace is not None and (not do_sample or top_k <= 32):
+        assert workspace.numel() >= lib().br_sample_logp_workspace_bytes(R, V), "logp needs sample_workspace(R, V, device, logp=True)"
+        check(lib().br_sample_next_2stage_logp(ptr(logits, "float*"), _row_major_2d(logits), R, V, float(temperature), int(top_k), float(top_p),
+                                               1 if do_sample else 0, ptr(uniforms, "float*"), ptr(step, "int32_t*"), int(max_steps), int(eos_id),
+                                               int(pad_id), ptr(finished, "int32_t*"), ptr(tokens, "int64_t*"), ptr(next_ids, "int64_t*"),
+                                               ptr(logp, "float*"), ptr(workspace), _stream()), "sample_next_2stage_logp")
+        return
+    check(lib().br_sample_next_logp(ptr(logits, "float*"), _row_major_2d(logits), R, V, float(temperature), int(top_k), float(top_p),
+                                    1 if do_sample else 0, ptr(uniforms, "float*"), ptr(step, "int32_t*"), int(max_steps), int(eos_id),
+                                    int(pad_id), ptr(finished, "int32_t*"), ptr(tokens, "int64_t*"), ptr(next_ids, "int64_t*"),
+                                    ptr(logp, "float*"), _stream()), "sample_next_logp")
 
 
 def decode_advance(step, cur_len):

@@ -74,3 +74,9 @@ class DNALLMGRPOConfig:
     suppress_eos: bool = False            # fixed-length rollouts (bench config c)
     share_prompt_prefix: bool = False     # ref / old / policy passes compute each prompt group's full prompt tiles once (same log-probs)
     fp8_rollout: bool = False             # rollout decode streams e4m3 layer weights (per-row scales); samples from the quantized policy
+    rollout_is_correction: bool = False   # weight each token's policy-gradient term by min(exp(old - rollout logp), rollout_is_cap)
+    rollout_is_cap: float = 2.0           # truncation of that importance weight (> 0; inf: untruncated)
+
+    def __post_init__(self):
+        if not (self.rollout_is_cap > 0):
+            raise ValueError(f"rollout_is_cap must be > 0 (inf for untruncated importance sampling), got {self.rollout_is_cap}")

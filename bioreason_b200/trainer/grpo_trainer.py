@@ -130,6 +130,9 @@ class DNALLMGRPOTrainer:
         # hard-coded exactly like grpo_trainer.py:384-391 (args.temperature/top_p/top_k are NOT consulted there either)
         self.generation_kwargs = dict(max_new_tokens=self.max_completion_length, do_sample=True, temperature=0.6, top_p=0.95, top_k=20,
                                       pad_token_id=self.pad_token_id, eos_token_id=None if a.suppress_eos else self.eos_token_id)
+        if getattr(a, "rollout_is_correction", False):
+            # the sampler's own log-probs of the tokens it drew (behaviour policy: merged / FP8 decode weights) for the IS weights
+            self.generation_kwargs["return_logprobs"] = True
         opt = optimizers[0]
         if opt is None:
             opt = torch.optim.AdamW(model.trainable_parameters(), lr=a.learning_rate, betas=(a.adam_beta1, a.adam_beta2), eps=a.adam_epsilon,
@@ -241,6 +244,9 @@ class DNALLMGRPOTrainer:
             uniforms = torch.rand(C, B, device=dev, generator=self._gen)
         with self._mark("rollout"):
             completion_ids = model.generate(prompt_ids, prompt_mask, mm["dna_tokenized"], mm["batch_idx_map"], uniforms=uniforms, **self.generation_kwargs)
+        sampling_lp = None
+        if self.generation_kwargs.get("return_logprobs"):
+            completion_ids, sampling_lp = completion_ids
         self.timings["rollout"] += time.perf_counter() - t0
         completion_mask = ops.eos_mask(completion_ids, self.eos_token_id if not self.args.suppress_eos else -1)      # :605-609
         # text reward functions need the ids on the host: start the copy now (side stream, pinned), wait for it only after the
@@ -274,9 +280,12 @@ class DNALLMGRPOTrainer:
         for i, f in enumerate(self.reward_funcs):
             self._metrics[f"rewards/{getattr(f, '__name__', 'reward_' + str(i))}"].append(rewards_all[:, i].mean())
         self.timings["score"] += time.perf_counter() - t0
-        return dict(prompt_ids=prompt_ids, prompt_mask=prompt_mask, completion_ids=completion_ids, completion_mask=completion_mask,
-                    old_per_token_logps=old_lp, ref_per_token_logps=ref_lp, advantages=advantages, multimodal_inputs=mm,
-                    local_group_size=gs)
+        out = dict(prompt_ids=prompt_ids, prompt_mask=prompt_mask, completion_ids=completion_ids, completion_mask=completion_mask,
+                   old_per_token_logps=old_lp, ref_per_token_logps=ref_lp, advantages=advantages, multimodal_inputs=mm,
+                   local_group_size=gs)
+        if sampling_lp is not None:
+            out["sampling_per_token_logps"] = sampling_lp
+        return out
 
     @staticmethod
     def _auto_micro_rows(model, B, L):
@@ -327,6 +336,14 @@ class DNALLMGRPOTrainer:
             mr = self.args.micro_rows or (self._auto_micro_rows(model, B, ids.shape[1]) if ids.is_cuda else B)
         ga = self.args.gradient_accumulation_steps
         loss_acc = torch.zeros(3, device=ids.device)
+        tis = getattr(self.args, "rollout_is_correction", False)
+        if tis:
+            samp = inputs.get("sampling_per_token_logps")
+            if samp is None:
+                raise ValueError("rollout_is_correction needs the rollout's log-probs: inputs lack 'sampling_per_token_logps' "
+                                 "(model.generate(..., return_logprobs=True))")
+            is_cap = getattr(self.args, "rollout_is_cap", 2.0)
+            is_acc = torch.zeros(4, device=ids.device)
         # one LoRA-dropout pass for all row chunks; each chunk passes its first row so the masks ignore the chunking
         pid = model.new_lora_dropout_pass() if getattr(model, "_lora", None) is not None else None
         for lo in range(0, B, mr):
@@ -338,10 +355,17 @@ class DNALLMGRPOTrainer:
                 drop_kw = dict(dropout=True, dropout_pass=pid, row_offset=lo) if pid is not None else {}
                 lp, ctx = training.policy_forward(model, ids[sl], mask[sl], mm_c["dna_tokenized"], mm_c["batch_idx_map"], C, save=backward,
                                                   **({"group_size": gs} if gs else {}), **drop_kw)
-            out3, dlp = ops.grpo_loss_raw(lp, old[sl] if old is not None else None, ref[sl] if ref is not None else None, adv[sl],
-                                          completion_mask[sl], self.beta, self.epsilon_low, self.epsilon_high, want_grad=backward)
+            if tis:
+                out3, is_stats, dlp = ops.grpo_loss_is_raw(lp, old[sl] if old is not None else None, ref[sl] if ref is not None else None,
+                                                           samp[sl], adv[sl], completion_mask[sl], self.beta, self.epsilon_low,
+                                                           self.epsilon_high, is_cap, want_grad=backward)
+            else:
+                out3, dlp = ops.grpo_loss_raw(lp, old[sl] if old is not None else None, ref[sl] if ref is not None else None, adv[sl],
+                                              completion_mask[sl], self.beta, self.epsilon_low, self.epsilon_high, want_grad=backward)
             w = (hi - lo) / B
             loss_acc += out3 * w                                            # row-mean of row-means is separable over row chunks
+            if tis:
+                is_acc += is_stats * w                                      # token means, row-weighted across chunks like clip_ratio
             self.timings["policy_fwd"] += time.perf_counter() - t0
             if backward:
                 t0 = time.perf_counter()
@@ -358,6 +382,9 @@ class DNALLMGRPOTrainer:
         if self.beta > 0:
             self._metrics["kl"].append(loss_acc[1])
         self._metrics["clip_ratio"].append(loss_acc[2])
+        if tis:
+            for name, v in zip(("ratio_mean", "capped_frac", "logp_diff", "kl"), is_acc):
+                self._metrics[f"rollout_is/{name}"].append(v)
         return loss_acc[0]
 
     # ------------------------------------------------------------------ one optimizer step

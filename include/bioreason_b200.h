@@ -43,6 +43,14 @@ int br_grpo_advantages(const float* rewards_per_func, int rows, int n_funcs, int
 int br_grpo_loss_fwd_bwd(const float* lp, const float* old_lp, const float* ref_lp, const float* adv,
                          const int32_t* mask, int B, int C, float beta, float eps_low, float eps_high,
                          float* out3, float* dlp, void* stream);
+/* The same loss with truncated importance sampling against the rollout: rollout_lp [B, C] f32 = the sampler's log-probs
+ * (br_sample_next*_logp).  Per token w = min(exp(o - rollout_lp), is_cap), o = old_lp (lp when NULL), a constant; the clipped
+ * policy-gradient term is multiplied by w, the KL term is not.  is_cap > 0 (+inf: untruncated).  out3 as above;
+ * is_stats[4] = masked token means of {w, [exp(o - rollout_lp) > is_cap], o - rollout_lp, exp(o - rollout_lp) - 1 - (o - rollout_lp)}.
+ * One launch. */
+int br_grpo_loss_is_fwd_bwd(const float* lp, const float* old_lp, const float* ref_lp, const float* rollout_lp, const float* adv,
+                            const int32_t* mask, int B, int C, float beta, float eps_low, float eps_high, float is_cap, float* out3,
+                            float* is_stats, float* dlp, void* stream);
 /* completion_mask[b, t] = t <= first_eos(b) (grpo_trainer.py:605-609); ids int64 [B, C] -> mask int32 */
 int br_eos_mask(const int64_t* completion_ids, int B, int C, int64_t eos_id, int32_t* mask, void* stream);
 
@@ -193,6 +201,17 @@ int64_t br_sample_workspace_bytes(int R, int V);
 int br_sample_next_2stage(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
                           const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id,
                           int32_t* finished, int64_t* tokens, int64_t* next_ids, void* workspace, void* stream);
+/* The two samplers above that also write the behaviour log-prob logp[r, step] (f32, laid out like tokens) = z[y] - logsumexp(z)
+ * over the raw logits row z (T = 1, full vocabulary, no top-k / top-p) at the chosen token y; finished rows write 0.  The
+ * two-stage one needs br_sample_logp_workspace_bytes(R, V): br_sample_workspace_bytes(R, V) followed by R * ceil(V / 4096)
+ * (max, sum exp) float pairs that stage 1 writes per chunk.  Tokens equal those of the calls without logp. */
+int64_t br_sample_logp_workspace_bytes(int R, int V);
+int br_sample_next_logp(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
+                        const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id, int32_t* finished,
+                        int64_t* tokens, int64_t* next_ids, float* logp, void* stream);
+int br_sample_next_2stage_logp(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
+                               const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id,
+                               int32_t* finished, int64_t* tokens, int64_t* next_ids, float* logp, void* workspace, void* stream);
 int br_decode_advance(int32_t* step, int32_t* cur_len, int R, void* stream);
 
 /* Decode attention, one launch per layer per step: per-head q/k RMSNorm + RoPE at cur_len[r], K/V append to the row's page,
