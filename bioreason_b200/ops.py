@@ -180,16 +180,21 @@ def lmhead_logprob(h: torch.Tensor, w: torch.Tensor, target: torch.Tensor, scale
     return logp, lse
 
 
-def lmhead_dlogits(h, w, target, lse, gscale, scale: float = 1.0):
-    """bf16 [M, V] tile-recomputed gradient of sum_m gscale[m] * logp[m] w.r.t. the logits."""
+def lmhead_dlogits(h, w, target, lse, gscale, scale: float = 1.0, out: Optional[torch.Tensor] = None):
+    """bf16 [M, V] tile-recomputed gradient of sum_m gscale[m] * logp[m] w.r.t. the logits.
+    out: optional bf16 [M, V] destination with contiguous rows (any row stride that is a multiple of 8)."""
     _need_cuda(h, w, target)
     M, K = h.shape
     V = w.shape[0]
     tgt = target.to(torch.int32).contiguous()
-    d = torch.empty(M, V, device=h.device, dtype=torch.bfloat16)
+    if out is None:
+        d = torch.empty(M, V, device=h.device, dtype=torch.bfloat16)
+    else:
+        assert out.dtype == torch.bfloat16 and out.shape == (M, V), (out.dtype, out.shape)
+        d = out
     check(lib().br_lmhead_dlogits(ptr(h), _row_major_2d(h), ptr(w), _row_major_2d(w), ptr(tgt, "int32_t*"),
                                   ptr(lse, "float*"), ptr(gscale.float().contiguous(), "float*"), M, V, K, float(scale),
-                                  ptr(d), V, _stream()), "lmhead_dlogits")
+                                  ptr(d), _row_major_2d(d), _stream()), "lmhead_dlogits")
     return d
 
 

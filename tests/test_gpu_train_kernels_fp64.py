@@ -26,13 +26,13 @@ def ops():
 
 
 def _bits(t):
-    return t.view(torch.int16)
+    return t.view(torch.int16 if t.element_size() == 2 else torch.int32)
 
 
-def _nan_buffer(rows, width, seed):
-    """bf16 [rows, width + PAD], NaN in the first `width` columns and a seeded sentinel pattern after them."""
-    buf = torch.full((rows, width + PAD), math.nan, dtype=torch.bfloat16, device="cuda")
-    buf[:, width:] = torch.randn(rows, PAD, generator=torch.Generator().manual_seed(seed)).to(torch.bfloat16).cuda()
+def _nan_buffer(rows, width, seed, dtype=torch.bfloat16):
+    """[rows, width + PAD] (bf16 or fp32), NaN in the first `width` columns and a seeded sentinel pattern after them."""
+    buf = torch.full((rows, width + PAD), math.nan, dtype=dtype, device="cuda")
+    buf[:, width:] = torch.randn(rows, PAD, generator=torch.Generator().manual_seed(seed)).to(dtype).cuda()
     return buf
 
 
