@@ -112,6 +112,25 @@ def plan_pages(plen: List[int], G: int, C: int):
     return dict(n_shared=n_shared, max_pages=max_pages, n_pages=nxt, table=table, prefill_pages=prefill_pages, tail_copies=tail_copies)
 
 
+DECODE_ITEMS_PER_SM = 3                 # CTAs of the fused attention an SM can hold (74 KB each)
+
+
+def decode_splits(R: int, G: int, Hkv: int, n_shared: int, n_sms: int):
+    """(splits_shared, splits_private) of the fused decode attention (host side, pure).  Two KV tiles per work item where the
+    co-residency cap allows it: both are fetched before the dependency wait, so the tile loop never waits on DRAM.  The in-kernel
+    merge needs every work item co-resident, so the splits are halved until (R / G) Hkv SS + R Hkv SP <= 3 n_sms."""
+    splits_shared = min(16, max(8, (n_shared + 1) // 2), n_shared) if n_shared > 0 else 0
+    splits_private = 3 if n_shared > 0 else 8
+    cap = DECODE_ITEMS_PER_SM * n_sms
+    n_items = lambda ss, sp: (R // G) * Hkv * ss + R * Hkv * sp
+    while n_items(splits_shared, splits_private) > cap and (splits_shared > 1 or splits_private > 1):
+        if splits_private > 1 and (splits_private >= splits_shared or splits_shared <= 1):
+            splits_private //= 2
+        else:
+            splits_shared = max(1, splits_shared // 2)
+    return splits_shared, splits_private
+
+
 class RolloutEngine:
     """Owns the KV page pool, decode scratch and the captured decode-step graph for one model."""
 
@@ -235,18 +254,7 @@ class RolloutEngine:
             St.cur_len = cur0.clone()
             St.uniforms = uniforms.clone() if params.do_sample else None
             St.scratch = ops.skinny_scratch(max(cfg.vocab_size, 2 * cfg.intermediate_size), dev)
-            # two KV tiles per work item where the co-residency cap allows it: both are fetched before the dependency wait, so the tile loop
-            # never waits on DRAM
-            splits_shared = min(16, max(8, (n_shared + 1) // 2), n_shared) if n_shared > 0 else 0
-            splits_private = 3 if n_shared > 0 else 8
-            per_sm = 3                                                                  # CTAs of the fused attention an SM can hold (74 KB each)
-            cap = per_sm * torch.cuda.get_device_properties(dev).multi_processor_count      # the fused kernel's merger items need co-residency
-            n_items = lambda ss, sp: (R // G) * Hkv * ss + R * Hkv * sp
-            while n_items(splits_shared, splits_private) > cap and (splits_shared > 1 or splits_private > 1):
-                if splits_private > 1 and (splits_private >= splits_shared or splits_shared <= 1):
-                    splits_private //= 2
-                else:
-                    splits_shared = max(1, splits_shared // 2)
+            splits_shared, splits_private = decode_splits(R, G, Hkv, n_shared, torch.cuda.get_device_properties(dev).multi_processor_count)
             if G * (Hq // Hkv) > 32:
                 raise NotImplementedError("fused decode attention handles G * Hq/Hkv <= 32 query vectors per kv head")
             St.splits = (splits_shared, splits_private)

@@ -1,7 +1,13 @@
 """Weight-only FP8 (e4m3) rollout decode: the per-row quantizer, the FP8 instantiation of the decode GEMM, the rollout plumbing and
 the trainer flag.  The e4m3 layout is private to the two kernels, so the codes are read back through the GEMM (one-hot X rows)."""
+import os
+import sys
+
 import pytest
 import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import decode_ref as dr  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -115,34 +121,11 @@ def _fp64_case(ops, scratch, R, N, K, mode, norm, seed, wrong=None):
     ssq_out = torch.full((((N + 127) // 128) * 4, 32), float("nan"), device="cuda") if want_ssq_out else None
     got = ops.skinny_gemm(x, fw, scratch, mode=mode, residual=res, sumsq_in=ssq, sumsq_in_n=n_part if norm else 1, sumsq_out=ssq_out,
                           eps=eps).double()
-    terms = (x.double().abs() @ wd.abs().T)                                 # sum |x w| per output
-    acc = x.double() @ wd.T
-    rs = torch.ones(R, 1, device="cuda", dtype=torch.float64)
-    if norm:
-        rs = (1.0 / torch.sqrt(ssq[:, :R].double().sum(0) / K + eps))[:, None]
-    v, tb = acc * rs, (2.0 ** -16 * terms + 2.0 ** -20 * acc.abs()) * rs      # fp32 accumulation + scale / rstd roundings
-    u8 = 2.0 ** -8                                                          # bf16 rounding (relative, with slack for the reference's)
-    if mode == 3:
-        ref, bound = v, tb
-    elif mode == 0:
-        ref, bound = v, tb + u8 * v.abs() + u8 * tb
-    elif mode == 1:
-        ref = v + res.double()
-        bound = tb + u8 * v.abs() + u8 * ref.abs() + 2 * u8 * tb
-    else:
-        G, U = v.view(R, N // 16, 2, 8)[:, :, 0], v.view(R, N // 16, 2, 8)[:, :, 1]
-        eg, eu = tb.view(R, N // 16, 2, 8)[:, :, 0], tb.view(R, N // 16, 2, 8)[:, :, 1]
-        sig = torch.sigmoid(G)
-        silu = G * sig
-        ref = (silu * U).reshape(R, N // 2)
-        dg = eg + u8 * G.abs()                                              # error of the bf16-rounded gate / up inputs
-        du = eu + u8 * U.abs()
-        bound = (1.1 * dg * (U.abs() + du) + silu.abs() * du + 2 * u8 * (silu.abs() + 1.1 * dg) * (U.abs() + du) + 1e-6 * silu.abs() * U.abs())
-        bound = bound.reshape(R, N // 2)
+    ref, bound = dr.skinny_ref(x, wd, mode, residual=res, sumsq_in=ssq, sumsq_in_n=n_part if norm else 1, eps=eps)
     err = (got - ref).abs()
     if wrong is None and want_ssq_out:
-        part = (got.float().double() ** 2).view(R, -1, 32).sum(2).T         # per 32 features, of the kernel's own bf16 outputs
-        torch.testing.assert_close(ssq_out[:, :R].double(), part, rtol=1e-5, atol=1e-6)
+        sref, sbound = dr.sumsq_out_ref(got, N)                             # of the kernel's own bf16 outputs
+        assert dr.worst_ratio(ssq_out[:, :R], sref, sbound) <= 1.0
     return (err / bound.clamp_min(1e-30)).max().item(), (err > bound).sum().item()
 
 

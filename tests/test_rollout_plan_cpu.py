@@ -63,3 +63,21 @@ def test_sampling_params_from_hf_kwargs():
     with pytest.raises(NotImplementedError, match="distinct eos_token_id"):                                        # never silently keep eos[0]
         SamplingParams.from_hf_kwargs(cfg, dict(eos_token_id=[11, 12]))
 
+
+
+@pytest.mark.parametrize("R,G,Hkv,n_shared,n_sms,want", [
+    (8, 8, 8, 28, 132, (14, 3)),          # config (c): one prompt x G = 8, 1852-token prompt
+    (32, 8, 8, 28, 132, (3, 1)),          # four groups: the shared splits halve to 7, then 3, then the private ones to 1
+    (8, 1, 8, 0, 132, (0, 4)),            # no sharing: 8 private splits would be 512 items > 396
+    (1, 1, 8, 0, 132, (0, 8)),
+    (16, 16, 8, 2, 132, (2, 1)),          # 16 + 384 = 400 items > 396: the private splits halve to 1
+    (4, 2, 8, 1, 132, (1, 3)),
+    (64, 8, 8, 28, 132, (1, 1)),          # nothing left to halve: the kernel's own argument check refuses the launch
+])
+def test_decode_splits(R, G, Hkv, n_shared, n_sms, want):
+    from bioreason_b200.generation import DECODE_ITEMS_PER_SM, decode_splits
+    ss, sp = decode_splits(R, G, Hkv, n_shared, n_sms)
+    assert (ss, sp) == want
+    assert ss <= n_shared and (ss == 0) == (n_shared == 0) and 1 <= sp and ss + sp <= 32
+    items = (R // G) * Hkv * ss + R * Hkv * sp
+    assert items <= DECODE_ITEMS_PER_SM * n_sms or (ss <= 1 and sp == 1)
