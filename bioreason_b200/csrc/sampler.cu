@@ -112,15 +112,17 @@ __device__ __forceinline__ float block_sum(float v, float* s_red) {
 // top_k-th value by radix select on shared-memory histograms and emits every element >= that value (value, token id) --
 // a superset of the row's global top-k.  Stage 2 (sampler_kernel, one CTA per row) then works on <= chunks*CAND_CAP
 // candidates instead of 151 936 logits: the sampler drops from ~200 us to ~20 us per decode step.
+// A chunk holding more than CAND_CAP finite values >= its k-th (only ties of the k-th can do that) emits the lowest-id CAND_CAP
+// and sets its overflow flag; stage 2 then selects on the logits row itself, so no tie HF keeps is lost.
 constexpr int CHUNK = 4096, CAND_CAP = 64;
 
 template <bool LOGP>
-__global__ void __launch_bounds__(256) sampler_partial_kernel(const float* __restrict__ logits, long long ld, int V, int top_k,
+__global__ void __launch_bounds__(256, 1) sampler_partial_kernel(const float* __restrict__ logits, long long ld, int V, int top_k,
                                                               float* __restrict__ cand_val, int* __restrict__ cand_idx, int n_chunks,
-                                                              float2* __restrict__ chunk_stats) {
+                                                              int* __restrict__ overflow, float2* __restrict__ chunk_stats) {
     __shared__ int hist[2048];
     __shared__ int s_tmp[4];
-    __shared__ int s_count;
+    __shared__ int s_count, s_ties;
     const int chunk = blockIdx.x, row = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     br::launch_dependents();
     br::grid_dep_wait();
@@ -180,6 +182,7 @@ __global__ void __launch_bounds__(256) sampler_partial_kernel(const float* __res
                 }
             }
             for (int s = cnt + tid; s < CAND_CAP; s += 256) { cv[s] = -INFINITY; ci[s] = 0x7fffffff; }
+            if (tid == 0) overflow[(long long)row * n_chunks + chunk] = 0;
             return;
         }
         __syncthreads();
@@ -214,8 +217,9 @@ __global__ void __launch_bounds__(256) sampler_partial_kernel(const float* __res
     }
     // values strictly above the k-th (fewer than k) always fit; ties OF the k-th fill the remaining slots in token-id order, so the
     // emitted set does not depend on the order in which threads reach an atomic
-    if (tid == 0) s_count = 0;
+    if (tid == 0) { s_count = 0; s_ties = 0; }
     __syncthreads();
+    int my_ties = 0;                                                   // finite ties only: -inf is never kept
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
         const int idx = base + i * 256 + tid;
@@ -223,8 +227,11 @@ __global__ void __launch_bounds__(256) sampler_partial_kernel(const float* __res
             const int s = atomicAdd(&s_count, 1);
             if (s < CAND_CAP) { cv[s] = v[i]; ci[s] = idx; }
         }
+        my_ties += idx < V && key[i] == prefix && v[i] > -INFINITY;
     }
+    if (my_ties) atomicAdd(&s_ties, my_ties);
     __syncthreads();
+    if (tid == 0) overflow[(long long)row * n_chunks + chunk] = s_count + s_ties > CAND_CAP;
     int filled = min(s_count, CAND_CAP);
     __shared__ int s_w[8];
 #pragma unroll
@@ -247,9 +254,14 @@ __global__ void __launch_bounds__(256) sampler_partial_kernel(const float* __res
 }
 
 // Stage 2 / single-stage sampler.  cand_idx == nullptr: x is the full logits row (index = position).
+// Stage 2 also gets the logits rows themselves (row_logits, row_ld, row_V) and stage 1's per-chunk overflow flags: when a chunk
+// dropped ties, or the candidates' ties of the k-th do not fit in MAXC, it selects on the row like the single-stage sampler.
+// Kept set: every value above the k-th plus its ties; past MAXC values in all, the ties with the lowest token ids.
 // LOGP: also writes logp[row, step]; chunk_stats = stage 1's n_chunks (m_c, s_c) pairs per row, or nullptr (single stage: x is the row).
 template <bool LOGP>
-__global__ void __launch_bounds__(1024) sampler_kernel(const float* __restrict__ logits, long long ld, int V, const int* __restrict__ cand_idx_all, float temperature, int top_k,
+__global__ void __launch_bounds__(1024, 1) sampler_kernel(const float* __restrict__ logits, long long ld, int V, const int* __restrict__ cand_idx_all,
+                                                       const float* __restrict__ row_logits, long long row_ld, int row_V,
+                                                       const int* __restrict__ overflow, float temperature, int top_k,
                                                        float top_p, int do_sample, const float* __restrict__ uniforms,
                                                        const int* __restrict__ step_ptr, int R, int max_steps, long long eos_id,
                                                        long long pad_id, int* __restrict__ finished, long long* __restrict__ tokens,
@@ -261,7 +273,7 @@ __global__ void __launch_bounds__(1024) sampler_kernel(const float* __restrict__
     __shared__ int c_idx[MAXC];
     __shared__ float o_val[MAXC];
     __shared__ int o_idx[MAXC];
-    __shared__ int s_count;
+    __shared__ int s_count, s_ties;
     __shared__ float r_val[32];
     __shared__ int r_idx[32];
     __shared__ float s_chosen_z;                                       // LOGP: the chosen token's raw logit
@@ -299,6 +311,7 @@ __global__ void __launch_bounds__(1024) sampler_kernel(const float* __restrict__
         choice = s_tmp[2];
     } else {
       bool fast_done = false;
+      int ovf = 0;                                                     // some stage-1 chunk of this row dropped ties (uniform)
       if (xi != nullptr && V <= 4 * (int)blockDim.x) {
         // ---- fast path over the stage-1 candidates (<= 4 per thread): superset by distance-to-maximum bins, exact ranking below
         float v[4]; int id[4]; int bin[4];
@@ -310,10 +323,12 @@ __global__ void __launch_bounds__(1024) sampler_kernel(const float* __restrict__
             v[i] = ok ? __ldcg(x + idx) : -INFINITY; id[i] = ok ? __ldcg(xi + idx) : 0x7fffffff;
             mx = fmaxf(mx, v[i]);
         }
+        int f = 0;
+        for (int c = tid; c < n_chunks; c += blockDim.x) f |= __ldcg(overflow + (long long)row * n_chunks + c);
         mx = block_max(mx, r_val);
         for (int i = tid; i < FBINS; i += blockDim.x) hist[i] = 0;
         if (tid == 0) s_count = 0;
-        __syncthreads();
+        ovf = __syncthreads_or(f);
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             bin[i] = v[i] > -INFINITY ? fast_bin(mx, v[i]) : FBINS - 1;
@@ -324,7 +339,7 @@ __global__ void __launch_bounds__(1024) sampler_kernel(const float* __restrict__
         __syncthreads();
         const int bstar = s_tmp[0], cnt = s_tmp[1];
         __syncthreads();
-        if (mx > -INFINITY && bstar >= 0 && cnt <= MAXC) {                       // uniform across the CTA
+        if (!ovf && mx > -INFINITY && bstar >= 0 && cnt <= MAXC) {              // uniform across the CTA
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 if (bin[i] <= bstar) { const int s = atomicAdd(&s_count, 1); c_val[s] = v[i]; c_idx[s] = id[i]; }
@@ -332,44 +347,97 @@ __global__ void __launch_bounds__(1024) sampler_kernel(const float* __restrict__
             fast_done = true;
         }
         __syncthreads();
+      } else if (xi != nullptr) {
+        int f = 0;
+        for (int c = tid; c < n_chunks; c += blockDim.x) f |= __ldcg(overflow + (long long)row * n_chunks + c);
+        ovf = __syncthreads_or(f);
       }
       if (!fast_done) {
-        // ---- exact k-th largest key by 3-pass radix select
-        uint32_t prefix = 0; int k_rem = top_k;
-        for (int pass = 0; pass < 3; ++pass) {
-            const int shift = pass == 0 ? 21 : (pass == 1 ? 10 : 0);
-            const int nb = pass == 2 ? 1024 : 2048;
-            for (int i = tid; i < 2048; i += blockDim.x) hist[i] = 0;
+        // candidates, or the logits row itself when the candidates may lack ties of the k-th
+        const float* src = x; const int* src_i = xi; int n = V;
+        if (ovf) { src = row_logits + (long long)row * row_ld; src_i = nullptr; n = row_V; }
+        for (;;) {                                                     // at most twice: candidates, then the row
+            const int k = min(top_k, n);                               // HF clamps top_k to the vocabulary
+            // ---- exact k-th largest key by 3-pass radix select
+            uint32_t prefix = 0; int k_rem = k;
+            for (int pass = 0; pass < 3; ++pass) {
+                const int shift = pass == 0 ? 21 : (pass == 1 ? 10 : 0);
+                const int nb = pass == 2 ? 1024 : 2048;
+                for (int i = tid; i < 2048; i += blockDim.x) hist[i] = 0;
+                __syncthreads();
+                for (int i = tid; i < n; i += blockDim.x) {
+                    const uint32_t key = fkey(__ldcg(src + i));
+                    bool in;
+                    if (pass == 0) in = true; else if (pass == 1) in = (key >> 21) == prefix; else in = (key >> 10) == prefix;
+                    if (in) atomicAdd(&hist[(key >> shift) & (nb - 1)], 1);
+                }
+                __syncthreads();
+                if (warp == 0) {
+                    int kr = k_rem;
+                    int b = find_bin(hist, nb, kr, s_tmp);
+                    if (lane == 0) { s_tmp[2] = b; s_tmp[3] = kr; }
+                }
+                __syncthreads();
+                const int b = s_tmp[2];
+                k_rem = s_tmp[3];
+                prefix = pass == 0 ? (uint32_t)b : (pass == 1 ? ((prefix << 11) | (uint32_t)b) : ((prefix << 10) | (uint32_t)b));
+                __syncthreads();
+            }
+            const uint32_t thr = prefix;
+            // values above the k-th (fewer than k) go to the front; its ties to the back while they fit beside them
+            const int tie_room = MAXC - k;
+            if (tid == 0) { s_count = 0; s_ties = 0; }
             __syncthreads();
-            for (int i = tid; i < V; i += blockDim.x) {
-                const uint32_t k = fkey(__ldcg(x + i));
-                bool in;
-                if (pass == 0) in = true; else if (pass == 1) in = (k >> 21) == prefix; else in = (k >> 10) == prefix;
-                if (in) atomicAdd(&hist[(k >> shift) & (nb - 1)], 1);
+            for (int i = tid; i < n; i += blockDim.x) {
+                const float v = __ldcg(src + i);
+                if (!(v > -INFINITY)) continue;
+                const uint32_t key = fkey(v);
+                if (key > thr) {
+                    const int s = atomicAdd(&s_count, 1);
+                    c_val[s] = v; c_idx[s] = src_i ? __ldcg(src_i + i) : i;
+                } else if (key == thr) {
+                    const int t = atomicAdd(&s_ties, 1);
+                    if (t < tie_room) { c_val[MAXC - 1 - t] = v; c_idx[MAXC - 1 - t] = src_i ? __ldcg(src_i + i) : i; }
+                }
             }
             __syncthreads();
-            if (warp == 0) {
-                int kr = k_rem;
-                int b = find_bin(hist, nb, kr, s_tmp);
-                if (lane == 0) { s_tmp[2] = b; s_tmp[3] = kr; }
+            const int n_above = s_count, n_tie = s_ties;
+            if (n_tie <= tie_room) {                                   // every tie collected: move them next to the values above
+                const bool mv = tid < n_tie;
+                float tv = 0.f; int ti = 0;
+                if (mv) { tv = c_val[MAXC - 1 - tid]; ti = c_idx[MAXC - 1 - tid]; }
+                __syncthreads();
+                if (mv) { c_val[n_above + tid] = tv; c_idx[n_above + tid] = ti; }
+                if (tid == 0) s_count = n_above + n_tie;
+                __syncthreads();
+                break;
             }
-            __syncthreads();
-            const int b = s_tmp[2];
-            k_rem = s_tmp[3];
-            prefix = pass == 0 ? (uint32_t)b : (pass == 1 ? ((prefix << 11) | (uint32_t)b) : ((prefix << 10) | (uint32_t)b));
-            __syncthreads();
+            if (src_i == nullptr) {
+                // more ties than room (the row itself: index = token id): fill with the lowest-id ties, so the kept set does not
+                // depend on the order in which threads reach an atomic
+                __shared__ int s_w[32];
+                const int nw = blockDim.x >> 5;
+                int filled = n_above;
+                for (int base = 0; base < n && filled < MAXC; base += blockDim.x) {       // uniform across the CTA
+                    const int i = base + tid;
+                    const float v = i < n ? __ldcg(src + i) : -INFINITY;
+                    const bool tie = v > -INFINITY && fkey(v) == thr;
+                    const unsigned m = __ballot_sync(0xffffffffu, tie);
+                    if (lane == 0) s_w[warp] = __popc(m);
+                    __syncthreads();
+                    int before = 0, total = 0;
+                    for (int w = 0; w < nw; ++w) { const int c = s_w[w]; total += c; if (w < warp) before += c; }
+                    const int slot = filled + before + __popc(m & ((1u << lane) - 1u));
+                    if (tie && slot < MAXC) { c_val[slot] = v; c_idx[slot] = i; }
+                    filled = min(MAXC, filled + total);
+                    __syncthreads();
+                }
+                if (tid == 0) s_count = filled;
+                __syncthreads();
+                break;
+            }
+            src = row_logits + (long long)row * row_ld; src_i = nullptr; n = row_V;   // candidate ties do not fit: select on the row
         }
-        const uint32_t thr = prefix;
-        if (tid == 0) s_count = 0;
-        __syncthreads();
-        for (int i = tid; i < V; i += blockDim.x) {
-            const float v = __ldcg(x + i);
-            if (fkey(v) >= thr && v > -INFINITY) {
-                const int s = atomicAdd(&s_count, 1);
-                if (s < MAXC) { c_val[s] = v; c_idx[s] = IDX(i); }
-            }
-        }
-        __syncthreads();
       }
         const int c_all = min(s_count, MAXC);
         // ---- rank sort: descending value, ties by ascending index
@@ -474,7 +542,7 @@ int br_sample_next(const float* logits, int64_t ld, int R, int V, float temperat
     if (do_sample) {
         BR_CHECK_ARG(temperature > 0.f && top_k >= 1 && top_k <= MAXC && top_p > 0.f && uniforms, "sample_next: need T > 0, 1 <= top_k <= %d, top_p > 0 and a uniforms buffer", MAXC);
     }
-    sampler_kernel<false><<<R, 1024, 0, (cudaStream_t)stream>>>(logits, ld, V, nullptr, temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps,
+    sampler_kernel<false><<<R, 1024, 0, (cudaStream_t)stream>>>(logits, ld, V, nullptr, nullptr, 0, 0, nullptr, temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps,
                                                                (long long)eos_id, (long long)pad_id, finished, (long long*)tokens, (long long*)next_ids,
                                                                nullptr, 0, nullptr);
     BR_CHECK_LAUNCH();
@@ -488,16 +556,19 @@ int br_sample_next_logp(const float* logits, int64_t ld, int R, int V, float tem
     if (do_sample) {
         BR_CHECK_ARG(temperature > 0.f && top_k >= 1 && top_k <= MAXC && top_p > 0.f && uniforms, "sample_next_logp: need T > 0, 1 <= top_k <= %d, top_p > 0 and a uniforms buffer", MAXC);
     }
-    sampler_kernel<true><<<R, 1024, 0, (cudaStream_t)stream>>>(logits, ld, V, nullptr, temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps,
+    sampler_kernel<true><<<R, 1024, 0, (cudaStream_t)stream>>>(logits, ld, V, nullptr, nullptr, 0, 0, nullptr, temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps,
                                                               (long long)eos_id, (long long)pad_id, finished, (long long*)tokens, (long long*)next_ids,
                                                               nullptr, 0, logp);
     BR_CHECK_LAUNCH();
     return BR_OK;
 }
 
+// workspace: candidate values and ids [R, n_chunks, CAND_CAP], then the chunks' overflow flags [R, n_chunks] (int, padded to 8 bytes)
+static int64_t flag_ints(int R, int n_chunks) { return ((int64_t)R * n_chunks + 1) & ~(int64_t)1; }
+
 int64_t br_sample_workspace_bytes(int R, int V) {
     const int n_chunks = (V + CHUNK - 1) / CHUNK;
-    return (int64_t)R * n_chunks * CAND_CAP * (sizeof(float) + sizeof(int));
+    return (int64_t)R * n_chunks * CAND_CAP * (sizeof(float) + sizeof(int)) + flag_ints(R, n_chunks) * sizeof(int);
 }
 
 int64_t br_sample_logp_workspace_bytes(int R, int V) {
@@ -516,18 +587,22 @@ static int sample_2stage(const float* logits, int64_t ld, int R, int V, float te
     float* cv = (float*)workspace;
     int* ci = (int*)(cv + (int64_t)R * n_chunks * CAND_CAP);
     cudaStream_t st = (cudaStream_t)stream;
+    int* flags = ci + (int64_t)R * n_chunks * CAND_CAP;
     const int n_cand = n_chunks * CAND_CAP;
     if (!logp) {
         BR_CHECK_CUDA(br_launch_pdl(sampler_partial_kernel<false>, dim3(n_chunks, R), dim3(256), 0, st, logits, (long long)ld, V, k, cv, ci, n_chunks,
-                                    (float2*)nullptr));
+                                    flags, (float2*)nullptr));
         BR_CHECK_CUDA(br_launch_pdl(sampler_kernel<false>, dim3(R), dim3(1024), 0, st, (const float*)cv, (long long)n_cand, n_cand, (const int*)ci,
+                                    logits, (long long)ld, V, (const int*)flags,
                                     temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps, (long long)eos_id, (long long)pad_id,
-                                    finished, (long long*)tokens, (long long*)next_ids, (const float2*)nullptr, 0, (float*)nullptr));
+                                    finished, (long long*)tokens, (long long*)next_ids, (const float2*)nullptr, n_chunks, (float*)nullptr));
         return BR_OK;
     }
-    float2* stats = (float2*)(ci + (int64_t)R * n_chunks * CAND_CAP);       // the tail of br_sample_logp_workspace_bytes
-    BR_CHECK_CUDA(br_launch_pdl(sampler_partial_kernel<true>, dim3(n_chunks, R), dim3(256), 0, st, logits, (long long)ld, V, k, cv, ci, n_chunks, stats));
+    float2* stats = (float2*)(flags + flag_ints(R, n_chunks));             // the tail of br_sample_logp_workspace_bytes
+    BR_CHECK_CUDA(br_launch_pdl(sampler_partial_kernel<true>, dim3(n_chunks, R), dim3(256), 0, st, logits, (long long)ld, V, k, cv, ci, n_chunks,
+                                flags, stats));
     BR_CHECK_CUDA(br_launch_pdl(sampler_kernel<true>, dim3(R), dim3(1024), 0, st, (const float*)cv, (long long)n_cand, n_cand, (const int*)ci,
+                                logits, (long long)ld, V, (const int*)flags,
                                 temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps, (long long)eos_id, (long long)pad_id,
                                 finished, (long long*)tokens, (long long*)next_ids, (const float2*)stats, n_chunks, logp));
     return BR_OK;

@@ -191,12 +191,15 @@ int br_scale_columns(void* W, int64_t ld, int64_t N, int K, const void* scale, v
 int br_kv_write_pages(const void* qkv, int64_t ld, int n_tok, int n_q_heads, int n_kv_heads, int head_dim, const int32_t* pages,
                       void* kcache, void* vcache, void* stream);
 /* temperature -> top-k -> top-p -> inverse-CDF draw with uniforms[step*R + r] (or argmax when !do_sample); finished rows
- * emit pad_id; writes tokens[r, step] (int64 [R, max_steps]) and next_ids[r]; eos_id < 0 disables EOS. */
+ * emit pad_id; writes tokens[r, step] (int64 [R, max_steps]) when step < max_steps and next_ids[r]; eos_id < 0 disables EOS.
+ * top_k is clamped to V; every value equal to the k-th is kept (HF's rule) up to 1024 kept values, past that the ties with the
+ * lowest token ids. */
 int br_sample_next(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
                    const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id, int32_t* finished,
                    int64_t* tokens, int64_t* next_ids, void* stream);
 /* Same semantics in two stages for large vocabularies: stage 1 (V/4096 CTAs per row) reduces each row to <= 64 candidates
- * per 4096-logit chunk, stage 2 samples from the candidates (top_k <= 32). */
+ * per 4096-logit chunk, stage 2 samples from the candidates (top_k <= 32), or from the logits row when a chunk held more ties
+ * of its k-th value than that.  The workspace holds the candidates and one overflow flag per chunk. */
 int64_t br_sample_workspace_bytes(int R, int V);
 int br_sample_next_2stage(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
                           const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id,
