@@ -7,12 +7,12 @@ project, regroup), :208-244 (merge + LLM forward).
 from __future__ import annotations
 
 from dataclasses import dataclass, field
-from typing import Callable, List, Optional
+from typing import Callable, Dict, List, Optional
 
 import torch
 
 from . import ops
-from .packing import DecoderW, EncoderW
+from .packing import LINEARS, DecoderLayerW, DecoderW, EncoderW, FusedLinear
 
 
 # ---------------------------------------------------------------------------------------------
@@ -45,22 +45,19 @@ def generate_positions(attention_mask: torch.Tensor) -> torch.Tensor:
 # LoRA adapters in kernel layout (packed from the fp32 master parameters each optimizer step)
 # ---------------------------------------------------------------------------------------------
 @dataclass
-class LoraLayerW:
-    a_qkv: torch.Tensor      # [3r, d]      rows = A_q | A_k | A_v
-    b_qkv: torch.Tensor      # [(Hq+2Hkv)D, 3r]  block diagonal
-    a_o: torch.Tensor        # [r, HqD]
-    b_o: torch.Tensor        # [d, r]
-    a_gu: torch.Tensor       # [2r, d]      rows = A_gate | A_up
-    b_gu: torch.Tensor       # [2F, 2r]     row 2j = (B_gate[j], 0), row 2j+1 = (0, B_up[j])
-    a_down: torch.Tensor     # [r, F]
-    b_down: torch.Tensor     # [d, r]
+class LoraLinearW:
+    """The adapters of one fused linear, laid out as packing.FusedLinear describes."""
+    a: torch.Tensor          # [n r, in]    rows = A of each target
+    b: torch.Tensor          # [out, n r]   block diagonal
+    a_T: torch.Tensor
+    b_T: torch.Tensor
 
 
 @dataclass
 class LoraW:
     r: int
     scale: float             # alpha / r, applied in the A-GEMM epilogue
-    layers: List[LoraLayerW]
+    layers: List[Dict[str, LoraLinearW]]      # per layer, keyed by FusedLinear.name
 
 
 @dataclass
@@ -89,10 +86,7 @@ class LayerSaved:
     xn2: torch.Tensor = None
     gu: torch.Tensor = None
     act: torch.Tensor = None
-    t_qkv: torch.Tensor = None
-    t_o: torch.Tensor = None
-    t_gu: torch.Tensor = None
-    t_down: torch.Tensor = None
+    t: Dict[str, torch.Tensor] = field(default_factory=dict)   # LoRA bottleneck x @ A.T of each fused linear
 
 
 _ROPE_TABLES = {}
@@ -107,13 +101,20 @@ def _rope_table(n_pos: int, D: int, theta: float, device):
     return t
 
 
-def _lin(x, w, *, lora_a=None, lora_b=None, lora_scale=1.0, saved_t=None, drop=None, **kw):
-    """y = x @ w.T (+ (scale * x @ A.T) @ B.T as a second K segment of the same wgmma accumulation).
-    drop: optional br_lora_dropout of this linear's projections: t = scale / (1 - p_eff) * (x * m_j) @ A_j.T; the base GEMM reads x."""
-    if lora_a is None:
-        return ops.gemm(x, w, **kw), None
-    t = ops.gemm(x, lora_a, alpha=lora_scale) if drop is None else ops.lora_down_dropout(x, lora_a, lora_scale, drop)
-    return ops.gemm(x, w, a2=t, b2=lora_b, **kw), t
+def _linear(f: FusedLinear, x, Lw: DecoderLayerW, li: int, lora: Optional[LoraW], dropout: Optional[LoraDropout], S, **kw):
+    """y = x @ w.T of fused linear f in layer li (+ (scale * x @ A.T) @ B.T as a second K segment of the same wgmma accumulation).
+    dropout: masks the adapter input per projection (ids f.proj0 + i): t = scale / (1 - p_eff) * (x * m_j) @ A_j.T; the base GEMM
+    reads x.  S (LayerSaved or None) keeps t for the backward."""
+    if lora is None:
+        return ops.gemm(x, getattr(Lw, f.name), **kw)
+    ad = lora.layers[li][f.name]
+    if dropout is None:
+        t = ops.gemm(x, ad.a, alpha=lora.scale)
+    else:
+        t = ops.lora_down_dropout(x, ad.a, lora.scale, ops.lora_dropout_desc(dropout, li, f.proj0, lora.r))
+    if S is not None:
+        S.t[f.name] = t
+    return ops.gemm(x, getattr(Lw, f.name), a2=t, b2=ad.b, **kw)
 
 
 def decoder_forward(W: DecoderW, h: torch.Tensor, B: int, L: int, positions: torch.Tensor, kv_start, kv_end, *,
@@ -132,31 +133,28 @@ def decoder_forward(W: DecoderW, h: torch.Tensor, B: int, L: int, positions: tor
     Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
     eps = cfg.rms_norm_eps
     theta = cfg.rope_parameters["rope_theta"] if hasattr(cfg, "rope_parameters") else cfg.rope_theta
-    qo, ko, vo = 0, Hq * D, (Hq + Hkv) * D
+    QKV, O, GU, DOWN = LINEARS
+    q_rows, k_rows, v_rows = QKV.rows(cfg)
     assert saved is None or kv_sink is None, "the KV sink reads roped K|V from the fused buffer; the training path keeps that buffer pre-norm"
     rope = _rope_table(L, D, theta, h.device)                          # cos/sin of positions 0..L-1, built once per (L, theta)
     for li, Lw in enumerate(W.layers):
-        lw = lora.layers[li] if lora is not None else None
-        ls = lora.scale if lora is not None else 1.0
-        dd = (lambda j: ops.lora_dropout_desc(dropout, li, j, lora.r)) if (dropout is not None and lw is not None) else (lambda j: None)
         S = LayerSaved() if saved is not None else None
         if S is not None:
             xn, rstd1 = ops.rmsnorm(h, Lw.ln1, eps, want_rstd=True)
             S.h_in, S.rstd1, S.xn1 = h, rstd1, xn
         else:
             xn = ops.rmsnorm(h, Lw.ln1, eps)
-        qkv, t = _lin(xn, Lw.w_qkv, lora_a=lw.a_qkv if lw else None, lora_b=lw.b_qkv if lw else None, lora_scale=ls, drop=dd(0))
+        qkv = _linear(QKV, xn, Lw, li, lora, dropout, S)
         if S is not None:
             # training: the roped q|k go to their own buffer, the GEMM output keeps the pre-norm q|k (qk-norm backward) and V -- no copy
-            S.t_qkv = t
             S.qkv_pre = qkv
-            qk = torch.empty(h.shape[0], vo, device=h.device, dtype=torch.bfloat16)
+            qk = torch.empty(h.shape[0], k_rows.stop, device=h.device, dtype=torch.bfloat16)
             ops.qk_rope_(qkv, Hq, Hkv, D, positions, theta, q_norm_w=Lw.q_norm, k_norm_w=Lw.k_norm, eps=eps, mode=0, out=qk, rope=rope)
-            q, k, v = qk[:, qo:ko], qk[:, ko:vo], qkv[:, vo:]
+            q, k, v = qk[:, q_rows], qk[:, k_rows], qkv[:, v_rows]
             S.q, S.k, S.v = q, k, v
         else:
             ops.qk_rope_(qkv, Hq, Hkv, D, positions, theta, q_norm_w=Lw.q_norm, k_norm_w=Lw.k_norm, eps=eps, mode=0, rope=rope)
-            q, k, v = qkv[:, qo:ko], qkv[:, ko:vo], qkv[:, vo:]
+            q, k, v = qkv[:, q_rows], qkv[:, k_rows], qkv[:, v_rows]
         if kv_sink is not None:
             kv_sink(li, qkv)
         if layout is not None:
@@ -171,21 +169,19 @@ def decoder_forward(W: DecoderW, h: torch.Tensor, B: int, L: int, positions: tor
             S.attn, S.lse = attn, lse
         else:
             attn = ops.attn_fwd(q, k, v, B, L, Hq, Hkv, D, kv_start=kv_start, kv_end=kv_end, causal=True)
-        h2, t = _lin(attn, Lw.w_o, lora_a=lw.a_o if lw else None, lora_b=lw.b_o if lw else None, lora_scale=ls, residual=h, drop=dd(3))
+        h2 = _linear(O, attn, Lw, li, lora, dropout, S, residual=h)
         if S is not None:
-            S.t_o = t
             xn2, rstd2 = ops.rmsnorm(h2, Lw.ln2, eps, want_rstd=True)
             S.h_mid, S.rstd2, S.xn2 = h2, rstd2, xn2
             gu = torch.empty(h.shape[0], Lw.w_gu.shape[0], device=h.device, dtype=torch.bfloat16)
         else:
             xn2 = ops.rmsnorm(h2, Lw.ln2, eps)
             gu = None
-        act, t = _lin(xn2, Lw.w_gu, lora_a=lw.a_gu if lw else None, lora_b=lw.b_gu if lw else None, lora_scale=ls, act=1, aux_out=gu, drop=dd(4))
+        act = _linear(GU, xn2, Lw, li, lora, dropout, S, act=1, aux_out=gu)
         if S is not None:
-            S.t_gu, S.gu, S.act = t, gu, act
-        h, t = _lin(act, Lw.w_down, lora_a=lw.a_down if lw else None, lora_b=lw.b_down if lw else None, lora_scale=ls, residual=h2, drop=dd(6))
+            S.gu, S.act = gu, act
+        h = _linear(DOWN, act, Lw, li, lora, dropout, S, residual=h2)
         if S is not None:
-            S.t_down = t
             saved.append(S)
     if not final_norm:
         return h

@@ -17,17 +17,15 @@ Dropout in decode would need unmerged adapters in the weight-streaming loop.
 """
 from __future__ import annotations
 
-import math
 from dataclasses import dataclass
 from typing import Dict, List
 
 import torch
 import torch.nn as nn
 
-from .engine import LoraDropout, LoraLayerW, LoraW
-from .packing import gu_views
-
-TARGETS = ("q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj")
+from . import ops
+from .engine import LoraDropout, LoraLinearW, LoraW
+from .packing import LINEARS, TARGETS, DecoderLayerW, DecoderW
 
 
 class LoraLinear(nn.Module):
@@ -70,8 +68,9 @@ class LoraState:
         self.modules: List[Dict[str, LoraLinear]] = []
         for layer in text_model.model.layers:
             mods = {}
-            for parent, names in ((layer.self_attn, ("q_proj", "k_proj", "v_proj", "o_proj")), (layer.mlp, ("gate_proj", "up_proj", "down_proj"))):
-                for n in names:
+            for f in LINEARS:
+                parent = getattr(layer, f.parent)
+                for n in f.targets:
                     lin = getattr(parent, n)
                     if not isinstance(lin, LoraLinear):
                         lin = LoraLinear(lin, r, alpha, g)
@@ -95,7 +94,7 @@ class LoraState:
         for p in self.params:
             self.grad_views.append(self.flat_grad[off:off + p.numel()].view_as(p))
             off += p.numel()
-        self._alloc_packed(dec_w, dev)
+        self._alloc_packed(dev)
         self.sync()
         self.dropout = None                # (p, threshold T, seed) while LoRA dropout is on
         self.dropout_pass = 0              # pass counter c of the masks: advanced once per dropout-applying pass
@@ -123,40 +122,30 @@ class LoraState:
         return LoraDropout(seed=seed, pass_id=pass_id, threshold=T, row_offset=row_offset)
 
     # ------------------------------------------------------------------
-    def _alloc_packed(self, W, dev):
-        cfg, r = self.cfg, self.r
-        d, F = cfg.hidden_size, cfg.intermediate_size
-        Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
-        nqkv = (Hq + 2 * Hkv) * D
-        bf = torch.bfloat16
-        z = lambda *s: torch.zeros(*s, device=dev, dtype=bf)
+    def _alloc_packed(self, dev):
+        r = self.r
+        z = lambda *s: torch.zeros(*s, device=dev, dtype=torch.bfloat16)
         self.w = LoraW(r=r, scale=self.scale, layers=[])
-        self.wT: List[Dict[str, torch.Tensor]] = []
         for _ in self.modules:
-            self.w.layers.append(LoraLayerW(a_qkv=z(3 * r, d), b_qkv=z(nqkv, 3 * r), a_o=z(r, Hq * D), b_o=z(d, r),
-                                            a_gu=z(2 * r, d), b_gu=z(2 * F, 2 * r), a_down=z(r, F), b_down=z(d, r)))
-            self.wT.append(dict(a_qkv_T=z(d, 3 * r), b_qkv_T=z(3 * r, nqkv), a_o_T=z(Hq * D, r), b_o_T=z(r, d),
-                                a_gu_T=z(d, 2 * r), b_gu_T=z(2 * r, 2 * F), a_down_T=z(F, r), b_down_T=z(r, d)))
+            layer = {}
+            for f in LINEARS:
+                (N, K), n = f.shape(self.cfg), len(f.targets) * r
+                layer[f.name] = LoraLinearW(a=z(n, K), b=z(N, n), a_T=z(K, n), b_T=z(n, N))
+            self.w.layers.append(layer)
 
     @torch.no_grad()
     def sync(self):
         """fp32 masters -> bf16 kernel layout (+ transposes).  Off-block entries of the block-diagonal B stay zero."""
-        cfg, r = self.cfg, self.r
-        Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
-        qo, ko, vo = 0, Hq * D, (Hq + Hkv) * D
-        for mods, L, T in zip(self.modules, self.w.layers, self.wT):
-            A = lambda n: mods[n].lora_A["default"].weight
-            B = lambda n: mods[n].lora_B["default"].weight
-            L.a_qkv[0:r].copy_(A("q_proj")); L.a_qkv[r:2 * r].copy_(A("k_proj")); L.a_qkv[2 * r:].copy_(A("v_proj"))
-            L.b_qkv[qo:ko, 0:r].copy_(B("q_proj")); L.b_qkv[ko:vo, r:2 * r].copy_(B("k_proj")); L.b_qkv[vo:, 2 * r:].copy_(B("v_proj"))
-            L.a_o.copy_(A("o_proj")); L.b_o.copy_(B("o_proj"))
-            L.a_gu[0:r].copy_(A("gate_proj")); L.a_gu[r:].copy_(A("up_proj"))
-            gv, uv = gu_views(L.b_gu)                                      # [F/8, 8, 2r] each
-            F = B("gate_proj").shape[0]
-            gv[..., 0:r].copy_(B("gate_proj").view(F // 8, 8, r)); uv[..., r:].copy_(B("up_proj").view(F // 8, 8, r))
-            L.a_down.copy_(A("down_proj")); L.b_down.copy_(B("down_proj"))
-            for k in ("a_qkv", "b_qkv", "a_o", "b_o", "a_gu", "b_gu", "a_down", "b_down"):
-                T[k + "_T"].copy_(getattr(L, k).t())
+        r = self.r
+        for mods, layer in zip(self.modules, self.w.layers):
+            for f in LINEARS:
+                ad = layer[f.name]
+                for i, n in enumerate(f.targets):
+                    ad.a[i * r:(i + 1) * r].copy_(mods[n].lora_A["default"].weight)
+                    dst = f.block(ad.b, i, self.cfg)[..., i * r:(i + 1) * r]
+                    dst.copy_(mods[n].lora_B["default"].weight.view(dst.shape))
+                ad.a_T.copy_(ad.a.t())
+                ad.b_T.copy_(ad.b.t())
 
     def zero_grad(self):
         self.flat_grad.zero_()
@@ -177,34 +166,27 @@ class LoraState:
         return self.grad_views[idx]
 
 
-# decode matrices whose input is RMS-normed: the norm gain is folded into their columns
-_FOLD = {"w_qkv": "ln1", "w_gu": "ln2"}
-_MATS = ("w_qkv", "w_o", "w_gu", "w_down")
-
-
-def _merge_into(dst, name, Lw, lora, i):
-    """dst <- W + scale * B A of decoder matrix `name` of layer i (W alone without adapters), then the norm gain folded in where
-    the input is normed."""
-    from . import ops
-    base = getattr(Lw, name)
+def _merge_into(dst, f, Lw, lora, i):
+    """dst <- W + scale * B A of fused linear f of layer i (W alone without adapters), then the norm gain folded in where the input
+    is normed."""
+    base = getattr(Lw, f.name)
     if lora is not None:
-        k = name[2:]
+        ad = lora.w.layers[i][f.name]
         # [N, K] = B[N, r'] @ (A^T)[K, r']^T ; K-major operands: A_op = B (K = r'), B_op = A^T ([K, r'])
-        ops.gemm(getattr(lora.w.layers[i], "b_" + k), lora.wT[i][f"a_{k}_T"], alpha=lora.scale, residual=base, out=dst)
+        ops.gemm(ad.b, ad.a_T, alpha=lora.scale, residual=base, out=dst)
     else:
         dst.copy_(base)
-    if name in _FOLD:
-        ops.scale_columns_(dst, getattr(Lw, _FOLD[name]))
+    if f.norm is not None:
+        ops.scale_columns_(dst, getattr(Lw, f.norm))
 
 
 def _rollout_shell(dec_w, make):
-    """DecoderW sharing the embedding, with its own final-norm-folded lm_head and per layer the matrices make(Lw, name) returns."""
-    from . import ops
-    from .packing import DecoderLayerW, DecoderW
+    """DecoderW sharing the embedding, with its own final-norm-folded lm_head and per layer the matrices make(Lw, f) returns."""
     out = DecoderW(cfg=dec_w.cfg, embed=dec_w.embed, lm_head=torch.empty_like(dec_w.lm_head), final_norm=dec_w.final_norm)
     out.folded = True
     for Lw in dec_w.layers:
-        out.layers.append(DecoderLayerW(ln1=Lw.ln1, ln2=Lw.ln2, q_norm=Lw.q_norm, k_norm=Lw.k_norm, **{n: make(Lw, n) for n in _MATS}))
+        out.layers.append(DecoderLayerW(ln1=Lw.ln1, ln2=Lw.ln2, q_norm=Lw.q_norm, k_norm=Lw.k_norm,
+                                        **{f.name: make(Lw, f) for f in LINEARS}))
     out.lm_head.copy_(dec_w.lm_head)
     ops.scale_columns_(out.lm_head, dec_w.final_norm)                      # frozen: folded once
     return out
@@ -217,13 +199,14 @@ def build_rollout_weights(dec_w, lora: "LoraState | None", out=None):
     consume a normed input (w_qkv <- ln1, w_gu <- ln2, lm_head <- final norm) so the decode step needs no norm launches."""
     if out is None:
         # without adapters w_o / w_down need neither a merge nor a fold: the frozen base matrices are used as they are
-        out = _rollout_shell(dec_w, lambda Lw, n: torch.empty_like(getattr(Lw, n)) if lora is not None or n in _FOLD else getattr(Lw, n))
+        out = _rollout_shell(dec_w, lambda Lw, f: torch.empty_like(getattr(Lw, f.name)) if lora is not None or f.norm is not None
+                             else getattr(Lw, f.name))
     for i, (Lw, Lo) in enumerate(zip(dec_w.layers, out.layers)):
-        if lora is not None and (Lo.w_o.data_ptr() == Lw.w_o.data_ptr() or Lo.w_down.data_ptr() == Lw.w_down.data_ptr()):
+        if lora is not None and any(getattr(Lo, f.name).data_ptr() == getattr(Lw, f.name).data_ptr() for f in LINEARS):
             raise RuntimeError("rollout weights alias the frozen base weights (built before enable_lora); rebuild them with out=None")
-        for n in _MATS:
-            if lora is not None or n in _FOLD:
-                _merge_into(getattr(Lo, n), n, Lw, lora, i)
+        for f in LINEARS:
+            if lora is not None or f.norm is not None:
+                _merge_into(getattr(Lo, f.name), f, Lw, lora, i)
     return out
 
 
@@ -232,19 +215,18 @@ def build_rollout_weights_fp8(dec_w, lora: "LoraState | None", out=None):
     """The decode weights of build_rollout_weights with the four layer matrices in weight-only FP8 (ops.Fp8Weight: e4m3 codes, one
     fp32 scale per output row); the embedding and the folded lm_head stay bf16.  Each matrix is merged and folded into one reusable
     bf16 scratch buffer (the largest matrix) and quantized from there, so no bf16 merged copy of the layers is kept."""
-    from . import ops
     if out is None:
         dev = dec_w.embed.device
-        out = _rollout_shell(dec_w, lambda Lw, n: ops.fp8_weight_empty(*getattr(Lw, n).shape, dev))
-        n_max = max(getattr(Lw, n).numel() for Lw in dec_w.layers for n in _MATS)
+        out = _rollout_shell(dec_w, lambda Lw, f: ops.fp8_weight_empty(*getattr(Lw, f.name).shape, dev))
+        n_max = max(getattr(Lw, f.name).numel() for Lw in dec_w.layers for f in LINEARS)
         out.fp8_scratch = torch.empty(n_max, device=dev, dtype=torch.bfloat16)
     for i, (Lw, Lo) in enumerate(zip(dec_w.layers, out.layers)):
-        for n in _MATS:
-            if lora is None and n not in _FOLD:
-                ops.quantize_rows_e4m3(getattr(Lw, n), out=getattr(Lo, n))
+        for f in LINEARS:
+            if lora is None and f.norm is None:
+                ops.quantize_rows_e4m3(getattr(Lw, f.name), out=getattr(Lo, f.name))
             else:
-                N, K = getattr(Lw, n).shape
+                N, K = getattr(Lw, f.name).shape
                 tmp = out.fp8_scratch[:N * K].view(N, K)
-                _merge_into(tmp, n, Lw, lora, i)
-                ops.quantize_rows_e4m3(tmp, out=getattr(Lo, n))
+                _merge_into(tmp, f, Lw, lora, i)
+                ops.quantize_rows_e4m3(tmp, out=getattr(Lo, f.name))
     return out

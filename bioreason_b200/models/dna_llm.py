@@ -22,7 +22,7 @@ import torch.nn as nn
 from .. import engine, ops
 from ..configs import dna_config as _dna_config
 from ..configs import text_config as _text_config
-from ..packing import gu_views, pack_decoder, pack_encoder, refresh_decoder_gu
+from ..packing import LINEARS, gu_views, pack_decoder, pack_encoder, refresh_decoder_gu
 
 _TEXT_ALIASES = {"Qwen/Qwen3-4B": "qwen3-4b", "Qwen/Qwen3-1.7B": "qwen3-1.7b"}
 _DNA_ALIASES = {"InstaDeepAI/nucleotide-transformer-v2-500m-multi-species": "nt-v2-500m"}
@@ -260,11 +260,11 @@ class DNALLMModel(nn.Module):
         (the merged model becomes the new frozen base / reference policy)."""
         if self._lora is None:
             return
-        from ..lora import TARGETS
         s = self._lora.scale
         for layer, mods in zip(self.text_model.model.layers, self._lora.modules):
-            for parent, names in ((layer.self_attn, TARGETS[:4]), (layer.mlp, TARGETS[4:])):
-                for n in names:
+            for f in LINEARS:
+                parent = getattr(layer, f.parent)
+                for n in f.targets:
                     ll = mods[n]
                     w = ll.base_layer.weight
                     w.data.add_((s * (ll.lora_B["default"].weight.float() @ ll.lora_A["default"].weight.float())).to(w.dtype))

@@ -113,7 +113,8 @@ def _row_major_2d(t):
 
 
 def lora_dropout_desc(drop, layer: int, proj: int, r: int):
-    """br_lora_dropout for projection `proj` (lora.TARGETS index; block i of a fused linear is proj + i) of decoder layer `layer`.
+    """br_lora_dropout for projection `proj` (packing.TARGETS index; block i of a fused linear is FusedLinear.proj0 + i, see
+    packing.LINEARS) of decoder layer `layer`.
     drop: engine.LoraDropout (seed, pass id, threshold, row offset)."""
     d = ffi.new("br_lora_dropout*")
     d.seed = int(drop.seed) & 0xFFFFFFFFFFFFFFFF

@@ -9,15 +9,67 @@ buffers laid out for the kernels:
                                            16-byte-aligned gate/up column groups for the backward kernels)
                   w_o   [d, Hq*D], w_down [d, F]
   encoder layer : w_qkv [3*d, d] (+ b_qkv), w_o, w_gu [2F, d] interleaved (x1_j, x2_j), w_down
-Frozen weights additionally get a transposed copy (`*_T`, [in, out]) so that the backward dX GEMMs are also
+Frozen weights additionally get a transposed copy (`w_T`, [in, out]) so that the backward dX GEMMs are also
 K-major x K-major (no MN-major descriptors); 180 GB of HBM makes the second copy (≈8 GB for Qwen3-4B) free.
+
+`LINEARS` is the one description of the decoder's fused linears: which peft projections each stacks and where their rows sit.
+Packing, the LoRA adapters' kernel layout, the forward and backward passes and the rollout merge all read it.
 """
 from __future__ import annotations
 
 from dataclasses import dataclass, field
-from typing import List, Optional
+from typing import Dict, List, Optional, Tuple
 
 import torch
+
+
+def proj_shape(cfg, target: str) -> Tuple[int, int]:
+    """(out_features, in_features) of one Qwen3 decoder projection."""
+    d, F, D = cfg.hidden_size, cfg.intermediate_size, cfg.head_dim
+    q, kv = cfg.num_attention_heads * D, cfg.num_key_value_heads * D
+    return {"q_proj": (q, d), "k_proj": (kv, d), "v_proj": (kv, d), "o_proj": (d, q),
+            "gate_proj": (F, d), "up_proj": (F, d), "down_proj": (d, F)}[target]
+
+
+@dataclass(frozen=True)
+class FusedLinear:
+    """One fused linear of a decoder layer.  Its LoRA adapters are packed the same way: A stacked by rows in target order
+    ([n r, in]), B block-diagonal ([out, n r]: target i's rows, columns i r .. (i+1) r)."""
+    name: str                    # the DecoderLayerW matrix
+    parent: str                  # HF module holding the projections
+    targets: Tuple[str, ...]     # peft targets, in packed order
+    blocked: bool = False        # rows in blocks of 8 | 8 (gate | up, gu_views) instead of one consecutive range per target
+    norm: Optional[str] = None   # DecoderLayerW norm gain folded into the columns of the decode copy (the input is RMS-normed)
+
+    @property
+    def proj0(self) -> int:
+        """LoRA dropout projection id of the first target (its TARGETS index); target i is proj0 + i."""
+        return TARGETS.index(self.targets[0])
+
+    def rows(self, cfg) -> List[slice]:
+        """Output rows of each target; a blocked linear interleaves its targets over all of its rows."""
+        outs = [proj_shape(cfg, t)[0] for t in self.targets]
+        if self.blocked:
+            return [slice(0, sum(outs))] * len(outs)
+        ends = [sum(outs[:i + 1]) for i in range(len(outs))]
+        return [slice(e - n, e) for e, n in zip(ends, outs)]
+
+    def shape(self, cfg) -> Tuple[int, int]:
+        """(out, in) of the fused matrix."""
+        return sum(proj_shape(cfg, t)[0] for t in self.targets), proj_shape(cfg, self.targets[0])[1]
+
+    def block(self, w: torch.Tensor, i: int, cfg) -> torch.Tensor:
+        """Target i's rows of a buffer laid out like this linear's output: [out_i, ...], or [out_i / 8, 8, ...] when blocked."""
+        return gu_views(w)[i] if self.blocked else w[self.rows(cfg)[i]]
+
+
+LINEARS = (
+    FusedLinear("w_qkv", "self_attn", ("q_proj", "k_proj", "v_proj"), norm="ln1"),
+    FusedLinear("w_o", "self_attn", ("o_proj",)),
+    FusedLinear("w_gu", "mlp", ("gate_proj", "up_proj"), blocked=True, norm="ln2"),
+    FusedLinear("w_down", "mlp", ("down_proj",)),
+)
+TARGETS = tuple(t for f in LINEARS for t in f.targets)     # LoRA dropout projection id = index; LoraState.params order
 
 
 def gu_views(w_gu: torch.Tensor):
@@ -25,19 +77,6 @@ def gu_views(w_gu: torch.Tensor):
     F2 = w_gu.shape[0]
     v = w_gu.view(F2 // 16, 2, 8, *w_gu.shape[1:])
     return v[:, 0], v[:, 1]
-
-
-def _repoint_gu(gate_p, up_p, w_gu):
-    F = gate_p.shape[0]
-    assert F % 8 == 0
-    gv, uv = gu_views(w_gu)
-    with torch.no_grad():
-        gv.copy_(gate_p.data.to(w_gu.dtype).view(F // 8, 8, -1))
-        uv.copy_(up_p.data.to(w_gu.dtype).view(F // 8, 8, -1))
-    # a [F, d] parameter cannot alias the blocked layout as one strided view; the container keeps its own (frozen)
-    # storage and `refresh_gu()` re-derives the kernel copy after a load_state_dict
-    gate_p.data = gate_p.data.to(device=w_gu.device, dtype=w_gu.dtype)
-    up_p.data = up_p.data.to(device=w_gu.device, dtype=w_gu.dtype)
 
 
 def _repoint(param: torch.nn.Parameter, view: torch.Tensor):
@@ -56,10 +95,7 @@ class DecoderLayerW:
     w_o: torch.Tensor
     w_gu: torch.Tensor
     w_down: torch.Tensor
-    w_qkv_T: Optional[torch.Tensor] = None
-    w_o_T: Optional[torch.Tensor] = None
-    w_gu_T: Optional[torch.Tensor] = None
-    w_down_T: Optional[torch.Tensor] = None
+    w_T: Optional[Dict[str, torch.Tensor]] = None     # transpose of each fused matrix, keyed by FusedLinear.name
 
 
 @dataclass
@@ -73,11 +109,8 @@ class DecoderW:
 
     def build_transposes(self):
         for L in self.layers:
-            if L.w_qkv_T is None:
-                L.w_qkv_T = L.w_qkv.t().contiguous()
-                L.w_o_T = L.w_o.t().contiguous()
-                L.w_gu_T = L.w_gu.t().contiguous()
-                L.w_down_T = L.w_down.t().contiguous()
+            if L.w_T is None:
+                L.w_T = {f.name: getattr(L, f.name).t().contiguous() for f in LINEARS}
         if self.lm_head_T is None:
             self.lm_head_T = self.lm_head.t().contiguous()
 
@@ -85,8 +118,7 @@ class DecoderW:
 def pack_decoder(model, device="cuda") -> DecoderW:
     """Fuse a HF Qwen3ForCausalLM's weights into kernel layout (bf16, on `device`) and re-point its parameters."""
     cfg = model.config
-    d, F = cfg.hidden_size, cfg.intermediate_size
-    Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+    d = cfg.hidden_size
     bf = torch.bfloat16
     emb_p = model.model.embed_tokens.weight
     embed = torch.empty(emb_p.shape, device=device, dtype=bf)
@@ -101,39 +133,44 @@ def pack_decoder(model, device="cuda") -> DecoderW:
     _repoint(model.model.norm.weight, fn)
     W = DecoderW(cfg=cfg, embed=embed, lm_head=lm_head, final_norm=fn)
     for layer in model.model.layers:
-        at, mlp = layer.self_attn, layer.mlp
-        w_qkv = torch.empty((Hq + 2 * Hkv) * D, d, device=device, dtype=bf)
-        _repoint(at.q_proj.weight, w_qkv[: Hq * D])
-        _repoint(at.k_proj.weight, w_qkv[Hq * D: (Hq + Hkv) * D])
-        _repoint(at.v_proj.weight, w_qkv[(Hq + Hkv) * D:])
-        w_o = torch.empty(d, Hq * D, device=device, dtype=bf)
-        _repoint(at.o_proj.weight, w_o)
-        w_gu = torch.empty(2 * F, d, device=device, dtype=bf)
-        _repoint_gu(mlp.gate_proj.weight, mlp.up_proj.weight, w_gu)
-        w_down = torch.empty(d, F, device=device, dtype=bf)
-        _repoint(mlp.down_proj.weight, w_down)
+        mats = {}
+        for f in LINEARS:
+            w = mats[f.name] = torch.empty(f.shape(cfg), device=device, dtype=bf)
+            for t, rows in zip(f.targets, f.rows(cfg)):
+                p = getattr(getattr(layer, f.parent), t).weight
+                if f.blocked:
+                    p.data = p.data.to(device=device, dtype=bf)             # own storage: _copy_blocked fills the kernel copy
+                else:
+                    _repoint(p, w[rows])
         small = {}
         for name, p in (("ln1", layer.input_layernorm.weight), ("ln2", layer.post_attention_layernorm.weight),
-                        ("q_norm", at.q_norm.weight), ("k_norm", at.k_norm.weight)):
+                        ("q_norm", layer.self_attn.q_norm.weight), ("k_norm", layer.self_attn.k_norm.weight)):
             t = torch.empty(p.shape, device=device, dtype=bf)
             _repoint(p, t)
             small[name] = t
-        W.layers.append(DecoderLayerW(w_qkv=w_qkv, w_o=w_o, w_gu=w_gu, w_down=w_down, **small))
+        W.layers.append(DecoderLayerW(**mats, **small))
+        _copy_blocked(layer, W.layers[-1], cfg)
     # buffers (rotary inv_freq) are not used by the kernels; leave them where they are
     return W
 
 
+def _copy_blocked(layer, Lw: DecoderLayerW, cfg):
+    """Blocked kernel copies (gate/up) from the container's parameters.  A [F, d] parameter cannot alias the blocked layout as one
+    strided view, so the container keeps its own (frozen) storage and refresh_decoder_gu re-derives the copy after a load."""
+    with torch.no_grad():
+        for f in LINEARS:
+            if f.blocked:
+                for i, t in enumerate(f.targets):
+                    dst = f.block(getattr(Lw, f.name), i, cfg)
+                    dst.copy_(getattr(getattr(layer, f.parent), t).weight.data.view(dst.shape))
+
+
 def refresh_decoder_gu(model, W: DecoderW):
     """Re-derive the blocked gate/up kernel copies from the container's gate_proj / up_proj (after loading weights)."""
-    with torch.no_grad():
-        for layer, Lw in zip(model.model.layers, W.layers):
-            gv, uv = gu_views(Lw.w_gu)
-            F = layer.mlp.gate_proj.weight.shape[0]
-            gv.copy_(layer.mlp.gate_proj.weight.data.view(F // 8, 8, -1))
-            uv.copy_(layer.mlp.up_proj.weight.data.view(F // 8, 8, -1))
-        for L in W.layers:
-            L.w_qkv_T = L.w_o_T = L.w_gu_T = L.w_down_T = None
-        W.lm_head_T = None
+    for layer, Lw in zip(model.model.layers, W.layers):
+        _copy_blocked(layer, Lw, W.cfg)
+        Lw.w_T = None
+    W.lm_head_T = None
 
 
 @dataclass

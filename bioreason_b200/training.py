@@ -14,7 +14,7 @@ import torch
 
 from . import engine, ops
 from .engine import LayerSaved
-from .lora import TARGETS
+from .packing import LINEARS
 
 
 class PolicyCtx:
@@ -175,7 +175,7 @@ def policy_backward(model, ctx: PolicyCtx, dlogp: torch.Tensor, on_layer_done=No
     W = model._dec
     W.build_transposes()
     cfg = W.cfg
-    Hq, Hkv, D, d, F = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim, cfg.hidden_size, cfg.intermediate_size
+    Hq, Hkv, D, d = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim, cfg.hidden_size
     theta = cfg.rope_parameters["rope_theta"] if hasattr(cfg, "rope_parameters") else cfg.rope_theta
     eps = cfg.rms_norm_eps
     B, L = ctx.B, ctx.L
@@ -185,7 +185,7 @@ def policy_backward(model, ctx: PolicyCtx, dlogp: torch.Tensor, on_layer_done=No
     lora = model._lora if ctx.use_lora else None
     r = lora.r if lora else 0
     s = lora.scale if lora else 1.0
-    qo, ko, vo = 0, Hq * D, (Hq + Hkv) * D
+    QKV, O, GU, DOWN = LINEARS
 
     # ---- lm_head: dlogits tiles recomputed from (h_sel, W) and the saved LSE, then dH = dlogits @ W
     g = dlogp.reshape(-1).float().contiguous()
@@ -200,67 +200,49 @@ def policy_backward(model, ctx: PolicyCtx, dlogp: torch.Tensor, on_layer_done=No
     drop = getattr(ctx, "drop", None)
 
     def dd(li, j):
-        """mask descriptor of projection j (lora.TARGETS index) in layer li, or None without dropout"""
+        """mask descriptor of projection j (packing.TARGETS index) in layer li, or None without dropout"""
         return ops.lora_dropout_desc(drop, li, j, r) if drop is not None else None
 
-    def lin_bwd(dy, w_T, x_in, t_saved, li, names, a_T, b_T, big_cols=None, **kw):
-        """dx = dy @ W (+ LoRA path) and LoRA grads.  names: LoRA target names fused in this linear (in packed order).
-        With dropout the u @ A segment is masked per projection: dx = dy @ W + sum_j m_j * inv_keep * (u_j @ A_j)."""
+    def linear_bwd(f, li, dy, x, S):
+        """dx = dy @ W of fused linear f (+ the LoRA path), then its adapter gradients.  With dropout the u @ A segment is masked per
+        projection: dx = dy @ W + sum_i m_i * inv_keep * (u_i @ A_i)."""
+        w_T = W.layers[li].w_T[f.name]
         if lora is None:
-            return ops.gemm(dy, w_T, **kw)
-        u = ops.gemm(dy, b_T, alpha=s)                                    # [M, r * len(names)] = s * dy @ B
-        dx = ops.gemm(dy, w_T, a2=u, b2=a_T, dropout=dd(li, TARGETS.index(names[0])), **kw)
-        return dx, u
+            return ops.gemm(dy, w_T)
+        ad = lora.w.layers[li][f.name]
+        u = ops.gemm(dy, ad.b_T, alpha=s)                                 # [M, n r] = s * dy @ B
+        dx = ops.gemm(dy, w_T, a2=u, b2=ad.a_T, dropout=dd(li, f.proj0))
+        # dB = dy^T t: one product over all of the linear's rows; each target keeps its rows and its own r columns (cross blocks are
+        # discarded).  Blocked rows (gate/up) take mode 2.
+        ops.lora_grad_tn(dy, S.t[f.name], [(lora.grad_view(li, t, "B"), rows.start, rows.stop, i * r, r)
+                                           for i, (t, rows) in enumerate(zip(f.targets, f.rows(cfg)))], mode=2 if f.blocked else 0)
+        for i, t in enumerate(f.targets):                                  # dA = u^T x
+            ops.lora_grad_tn(x, u[:, i * r:(i + 1) * r], [(lora.grad_view(li, t, "A"), 0, x.shape[1], 0, r)], mode=1,
+                             dropout=dd(li, f.proj0 + i))
+        return dx
 
     for li in range(len(W.layers) - 1, -1, -1):
         Lw, S = W.layers[li], ctx.saved[li]
-        Tl = lora.wT[li] if lora else None
         # ---------------- MLP: h_out = h_mid + down(act)
-        if lora:
-            dact, u = lin_bwd(dh, Lw.w_down_T, S.act, S.t_down, li, ("down_proj",), Tl["a_down_T"], Tl["b_down_T"])
-            ops.lora_grad_tn(dh, S.t_down, [(lora.grad_view(li, "down_proj", "B"), 0, d, 0, r)])               # dB = dy^T t
-            ops.lora_grad_tn(S.act, u, [(lora.grad_view(li, "down_proj", "A"), 0, F, 0, r)], mode=1, dropout=dd(li, 6))  # dA = u^T x
-        else:
-            dact = ops.gemm(dh, Lw.w_down_T)
+        dact = linear_bwd(DOWN, li, dh, S.act, S)
         dgu = ops.swiglu_bwd(S.gu, dact)
         del dact
-        if lora:
-            dxn2, u = lin_bwd(dgu, Lw.w_gu_T, S.xn2, S.t_gu, li, ("gate_proj", "up_proj"), Tl["a_gu_T"], Tl["b_gu_T"])
-            # one product dgu^T [2F] x t_gu [2r]: gate rows keep their r columns, up rows theirs (cross blocks are discarded)
-            ops.lora_grad_tn(dgu, S.t_gu, [(lora.grad_view(li, "gate_proj", "B"), 0, 2 * F, 0, r),
-                                           (lora.grad_view(li, "up_proj", "B"), 0, 2 * F, r, r)], mode=2)
-            ops.lora_grad_tn(S.xn2, u[:, :r], [(lora.grad_view(li, "gate_proj", "A"), 0, d, 0, r)], mode=1, dropout=dd(li, 4))
-            ops.lora_grad_tn(S.xn2, u[:, r:], [(lora.grad_view(li, "up_proj", "A"), 0, d, 0, r)], mode=1, dropout=dd(li, 5))
-        else:
-            dxn2 = ops.gemm(dgu, Lw.w_gu_T)
+        dxn2 = linear_bwd(GU, li, dgu, S.xn2, S)
         del dgu
         dh_mid = ops.rmsnorm_bwd(S.h_mid, Lw.ln2, S.rstd2, dxn2, dres=dh)
         del dxn2
         # ---------------- attention: h_mid = h_in + o_proj(attn)
-        if lora:
-            dattn, u = lin_bwd(dh_mid, Lw.w_o_T, S.attn, S.t_o, li, ("o_proj",), Tl["a_o_T"], Tl["b_o_T"])
-            ops.lora_grad_tn(dh_mid, S.t_o, [(lora.grad_view(li, "o_proj", "B"), 0, d, 0, r)])
-            ops.lora_grad_tn(S.attn, u, [(lora.grad_view(li, "o_proj", "A"), 0, Hq * D, 0, r)], mode=1, dropout=dd(li, 3))
-        else:
-            dattn = ops.gemm(dh_mid, Lw.w_o_T)
+        dattn = linear_bwd(O, li, dh_mid, S.attn, S)
         dqkv = torch.empty(M, (Hq + 2 * Hkv) * D, device=dev, dtype=torch.bfloat16)
+        dq, dk, dv = (dqkv[:, rows] for rows in QKV.rows(cfg))
         if layout is None:
-            ops.attn_bwd(S.q, S.k, S.v, S.attn, dattn, S.lse, dqkv[:, qo:ko], dqkv[:, ko:vo], dqkv[:, vo:],
-                         B, L, Hq, Hkv, D, kv_start=ctx.ks, kv_end=ctx.ke)
+            ops.attn_bwd(S.q, S.k, S.v, S.attn, dattn, S.lse, dq, dk, dv, B, L, Hq, Hkv, D, kv_start=ctx.ks, kv_end=ctx.ke)
         else:
-            ops.attn_bwd_shared(S.q, S.k, S.v, S.attn, dattn, S.lse, dqkv[:, qo:ko], dqkv[:, ko:vo], dqkv[:, vo:], layout.U, layout.G,
-                                layout.Lp, layout.Ls, Hq, Hkv, D, layout.kv_start, layout.kv_end)
+            ops.attn_bwd_shared(S.q, S.k, S.v, S.attn, dattn, S.lse, dq, dk, dv, layout.U, layout.G, layout.Lp, layout.Ls, Hq, Hkv, D,
+                                layout.kv_start, layout.kv_end)
         del dattn
         ops.qk_rope_bwd_(dqkv, S.qkv_pre, Hq, Hkv, D, Lw.q_norm, Lw.k_norm, ctx.pos, theta, eps)
-        if lora:
-            dxn1, u = lin_bwd(dqkv, Lw.w_qkv_T, S.xn1, S.t_qkv, li, ("q_proj", "k_proj", "v_proj"), Tl["a_qkv_T"], Tl["b_qkv_T"])
-            # one product dqkv^T [(Hq+2Hkv)D] x t_qkv [3r]: the q / k / v row blocks keep their own r columns
-            ops.lora_grad_tn(dqkv, S.t_qkv, [(lora.grad_view(li, "q_proj", "B"), qo, ko, 0, r), (lora.grad_view(li, "k_proj", "B"), ko, vo, r, r),
-                                             (lora.grad_view(li, "v_proj", "B"), vo, vo + Hkv * D, 2 * r, r)])
-            for j, name in enumerate(("q_proj", "k_proj", "v_proj")):
-                ops.lora_grad_tn(S.xn1, u[:, j * r:(j + 1) * r], [(lora.grad_view(li, name, "A"), 0, d, 0, r)], mode=1, dropout=dd(li, j))
-        else:
-            dxn1 = ops.gemm(dqkv, Lw.w_qkv_T)
+        dxn1 = linear_bwd(QKV, li, dqkv, S.xn1, S)
         del dqkv
         dh = ops.rmsnorm_bwd(S.h_in, Lw.ln1, S.rstd1, dxn1, dres=dh_mid)
         del dxn1, dh_mid
