@@ -8,6 +8,7 @@
 // cum <= 1 - p, always keep the best).  The draw is inverse-CDF over the kept tokens in ascending token id with a
 // caller-supplied uniform per (step, row): torch.multinomial's Philox consumption cannot be reproduced outside
 // torch, so parity is defined on supplied uniforms (SURVEY.md §7 "Sampling parity").
+// The *_proc entry points add HF's repetition penalty and min_new_tokens ahead of the warpers and min-p after top-p (see Proc below).
 #include "br_common.cuh"
 #include "../../include/bioreason_b200.h"
 
@@ -116,10 +117,33 @@ __device__ __forceinline__ float block_sum(float v, float* s_red) {
 // and sets its overflow flag; stage 2 then selects on the logits row itself, so no tie HF keeps is lost.
 constexpr int CHUNK = 4096, CAND_CAP = 64;
 
-template <bool LOGP>
+// Processed path (the *_proc entry points, PROC = true): HF's RepetitionPenalty -> MinNewTokens logits processors ahead of temperature /
+// top-k / top-p, and MinP after top-p.  Every kernel that reads a logit of the row applies proc_logit to it (stage 1 to the 16 values it
+// holds in registers, stage 2 and the single-stage sampler wherever they select on the row itself), so the candidates carry processed
+// values.  The log-prob stays on the raw row.  presence[r] is a bitmap of the tokens row r has emitted (bit j of word j / 32); the
+// sampler sets the emitted token's bit after the draw, one writer per row.
+struct Proc {
+    uint32_t* presence;           // [R, ceil(V / 32)], or nullptr: no penalty and no update
+    float theta;                  // repetition penalty
+    float min_p;                  // 0: off
+    int min_new;                  // EOS gets -inf while *step < min_new
+    long long eos;                // < 0: no EOS
+    const int* step;              // nullptr: step 0
+};
+
+// HF RepetitionPenaltyLogitsProcessor (z < 0 ? z * theta : z / theta, fp32, IEEE division) then MinNewTokensLengthLogitsProcessor
+__device__ __forceinline__ float proc_logit(float z, bool in_set, bool blocked, float theta) {
+    if (in_set) z = z < 0.f ? __fmul_rn(z, theta) : __fdiv_rn(z, theta);
+    return blocked ? -INFINITY : z;
+}
+__device__ __forceinline__ bool proc_in_set(const uint32_t* pres, int id) {
+    return pres != nullptr && ((__ldcg(pres + (id >> 5)) >> (id & 31)) & 1u);
+}
+
+template <bool LOGP, bool PROC>
 __global__ void __launch_bounds__(256, 1) sampler_partial_kernel(const float* __restrict__ logits, long long ld, int V, int top_k,
                                                               float* __restrict__ cand_val, int* __restrict__ cand_idx, int n_chunks,
-                                                              int* __restrict__ overflow, float2* __restrict__ chunk_stats) {
+                                                              int* __restrict__ overflow, float2* __restrict__ chunk_stats, Proc pr) {
     __shared__ int hist[2048];
     __shared__ int s_tmp[4];
     __shared__ int s_count, s_ties;
@@ -138,6 +162,35 @@ __global__ void __launch_bounds__(256, 1) sampler_partial_kernel(const float* __
         key[i] = ok ? fkey(v[i]) : 0u;
         n_valid += ok;
     }
+    if constexpr (PROC) {
+        if constexpr (LOGP) {
+            // the chunk statistics of the log-prob come from the raw values
+            __shared__ float s_red_raw[32];
+            float mr = -INFINITY;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) mr = fmaxf(mr, v[i]);
+            mr = block_max(mr, s_red_raw);
+            float s = 0.f;
+            if (mr > -INFINITY) {
+#pragma unroll
+                for (int i = 0; i < 16; ++i) s += expf(v[i] - mr);
+            }
+            s = block_sum(s, s_red_raw);
+            if (tid == 0) chunk_stats[(long long)row * n_chunks + chunk] = make_float2(mr, s);
+        }
+        // a warp's 32 consecutive ids share one bitmap word: one broadcast load per i
+        const int step = pr.step ? __ldcg(pr.step) : 0;
+        const bool block_eos = pr.eos >= 0 && step < pr.min_new;
+        const uint32_t* pres = pr.presence ? pr.presence + (long long)row * ((V + 31) >> 5) : nullptr;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            const int idx = base + i * 256 + tid;
+            if (idx < V) {
+                v[i] = proc_logit(v[i], proc_in_set(pres, idx), block_eos && idx == pr.eos, pr.theta);
+                key[i] = fkey(v[i]);
+            }
+        }
+    }
     const int n_here = min(CHUNK, V - base);
     const int k = min(top_k, n_here);
     float* cv = cand_val + ((long long)row * n_chunks + chunk) * CAND_CAP;
@@ -149,7 +202,7 @@ __global__ void __launch_bounds__(256, 1) sampler_partial_kernel(const float* __
 #pragma unroll
         for (int i = 0; i < 16; ++i) mx = fmaxf(mx, v[i]);
         mx = block_max(mx, s_red);
-        if constexpr (LOGP) {
+        if constexpr (LOGP && !PROC) {
             // (m_c, s_c) before the fast / exact split (the fast path returns early); entries past V hold -inf and add 0, and an
             // all -inf chunk gives (-inf, 0)
             float s = 0.f;
@@ -258,7 +311,7 @@ __global__ void __launch_bounds__(256, 1) sampler_partial_kernel(const float* __
 // dropped ties, or the candidates' ties of the k-th do not fit in MAXC, it selects on the row like the single-stage sampler.
 // Kept set: every value above the k-th plus its ties; past MAXC values in all, the ties with the lowest token ids.
 // LOGP: also writes logp[row, step]; chunk_stats = stage 1's n_chunks (m_c, s_c) pairs per row, or nullptr (single stage: x is the row).
-template <bool LOGP>
+template <bool LOGP, bool PROC>
 __global__ void __launch_bounds__(1024, 1) sampler_kernel(const float* __restrict__ logits, long long ld, int V, const int* __restrict__ cand_idx_all,
                                                        const float* __restrict__ row_logits, long long row_ld, int row_V,
                                                        const int* __restrict__ overflow, float temperature, int top_k,
@@ -266,7 +319,7 @@ __global__ void __launch_bounds__(1024, 1) sampler_kernel(const float* __restric
                                                        const int* __restrict__ step_ptr, int R, int max_steps, long long eos_id,
                                                        long long pad_id, int* __restrict__ finished, long long* __restrict__ tokens,
                                                        long long* __restrict__ next_ids, const float2* __restrict__ chunk_stats, int n_chunks,
-                                                       float* __restrict__ logp) {
+                                                       float* __restrict__ logp, Proc pr) {
     __shared__ int hist[2048];
     __shared__ int s_tmp[4];
     __shared__ float c_val[MAXC];
@@ -286,10 +339,23 @@ __global__ void __launch_bounds__(1024, 1) sampler_kernel(const float* __restric
     auto IDX = [&](int i) { return xi ? __ldcg(xi + i) : i; };
     const int step = step_ptr ? __ldcg(step_ptr) : 0;
     long long choice;
+    // PROC: the row itself (single stage, or stage 2's fallback) is read through proc_logit; the candidates already carry processed values
+    const int rowV = xi ? row_V : V;
+    const uint32_t* pres = nullptr;
+    bool block_eos = false;
+    if constexpr (PROC) {
+        pres = pr.presence ? pr.presence + (long long)row * ((rowV + 31) >> 5) : nullptr;
+        block_eos = pr.eos >= 0 && step < pr.min_new;
+    }
+    auto PZ = [&](float z, int id) { return proc_logit(z, proc_in_set(pres, id), block_eos && id == pr.eos, pr.theta); };
 
     if (!do_sample) {
         float bv = -INFINITY; int bi = 0x7fffffff;
-        for (int i = tid; i < V; i += blockDim.x) { float v = __ldcg(x + i); const int id = IDX(i); if (v > bv || (v == bv && id < bi)) { bv = v; bi = id; } }
+        for (int i = tid; i < V; i += blockDim.x) {
+            float v = __ldcg(x + i); const int id = IDX(i);
+            if constexpr (PROC) { if (!xi) v = PZ(v, i); }
+            if (v > bv || (v == bv && id < bi)) { bv = v; bi = id; }
+        }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
             float ov = __shfl_xor_sync(0xffffffffu, bv, o); int oi = __shfl_xor_sync(0xffffffffu, bi, o);
@@ -366,7 +432,9 @@ __global__ void __launch_bounds__(1024, 1) sampler_kernel(const float* __restric
                 for (int i = tid; i < 2048; i += blockDim.x) hist[i] = 0;
                 __syncthreads();
                 for (int i = tid; i < n; i += blockDim.x) {
-                    const uint32_t key = fkey(__ldcg(src + i));
+                    float zv = __ldcg(src + i);
+                    if constexpr (PROC) { if (!src_i) zv = PZ(zv, i); }
+                    const uint32_t key = fkey(zv);
                     bool in;
                     if (pass == 0) in = true; else if (pass == 1) in = (key >> 21) == prefix; else in = (key >> 10) == prefix;
                     if (in) atomicAdd(&hist[(key >> shift) & (nb - 1)], 1);
@@ -389,7 +457,8 @@ __global__ void __launch_bounds__(1024, 1) sampler_kernel(const float* __restric
             if (tid == 0) { s_count = 0; s_ties = 0; }
             __syncthreads();
             for (int i = tid; i < n; i += blockDim.x) {
-                const float v = __ldcg(src + i);
+                float v = __ldcg(src + i);
+                if constexpr (PROC) { if (!src_i) v = PZ(v, i); }
                 if (!(v > -INFINITY)) continue;
                 const uint32_t key = fkey(v);
                 if (key > thr) {
@@ -420,7 +489,8 @@ __global__ void __launch_bounds__(1024, 1) sampler_kernel(const float* __restric
                 int filled = n_above;
                 for (int base = 0; base < n && filled < MAXC; base += blockDim.x) {       // uniform across the CTA
                     const int i = base + tid;
-                    const float v = i < n ? __ldcg(src + i) : -INFINITY;
+                    float v = i < n ? __ldcg(src + i) : -INFINITY;
+                    if constexpr (PROC) { if (i < n) v = PZ(v, i); }
                     const bool tie = v > -INFINITY && fkey(v) == thr;
                     const unsigned m = __ballot_sync(0xffffffffu, tie);
                     if (lane == 0) s_w[warp] = __popc(m);
@@ -468,6 +538,13 @@ __global__ void __launch_bounds__(1024, 1) sampler_kernel(const float* __restric
                     if (cum <= lim) keep = j; else break;
                 }
             }
+            if constexpr (PROC) {
+                // min-p (HF MinPLogitsWarper, after top-p): drop p_j < min_p p_max, i.e. e_j = exp((z_j - z_max) / T) < min_p; the
+                // maximum always stays
+                if (pr.min_p > 0.f) {
+                    for (int j = 1; j < keep; ++j) if (c_val[j] < pr.min_p) { keep = j; break; }
+                }
+            }
             float ktot = 0.f;
             for (int j = 0; j < keep; ++j) ktot += c_val[j];
             // inverse CDF in ascending token id
@@ -511,6 +588,12 @@ __global__ void __launch_bounds__(1024, 1) sampler_kernel(const float* __restric
             lse = m + logf(block_sum(s, r_val));
         }
     }
+    if constexpr (LOGP && PROC) {
+        if (tid == 0) {                                                // the log-prob reads the raw logit of the chosen token
+            const float* zr = xi ? row_logits + (long long)row * row_ld : x;
+            s_chosen_z = (choice >= 0 && choice < rowV) ? __ldcg(zr + choice) : -INFINITY;
+        }
+    }
     if (tid == 0) {
         const int fin = finished ? __ldcg(finished + row) : 0;
         long long tok = fin ? pad_id : choice;                         // finished rows emit pad (HF :2796-2797)
@@ -518,6 +601,9 @@ __global__ void __launch_bounds__(1024, 1) sampler_kernel(const float* __restric
         if constexpr (LOGP) { if (step < max_steps) logp[(long long)row * max_steps + step] = fin ? 0.f : s_chosen_z - lse; }
         if (next_ids) next_ids[row] = tok;
         if (finished && !fin && eos_id >= 0 && tok == eos_id) finished[row] = 1;
+        if constexpr (PROC) {
+            if (pr.presence && tok >= 0 && tok < rowV) pr.presence[(long long)row * ((rowV + 31) >> 5) + (tok >> 5)] |= 1u << (tok & 31);
+        }
     }
 }
 
@@ -542,9 +628,9 @@ int br_sample_next(const float* logits, int64_t ld, int R, int V, float temperat
     if (do_sample) {
         BR_CHECK_ARG(temperature > 0.f && top_k >= 1 && top_k <= MAXC && top_p > 0.f && uniforms, "sample_next: need T > 0, 1 <= top_k <= %d, top_p > 0 and a uniforms buffer", MAXC);
     }
-    sampler_kernel<false><<<R, 1024, 0, (cudaStream_t)stream>>>(logits, ld, V, nullptr, nullptr, 0, 0, nullptr, temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps,
-                                                               (long long)eos_id, (long long)pad_id, finished, (long long*)tokens, (long long*)next_ids,
-                                                               nullptr, 0, nullptr);
+    sampler_kernel<false, false><<<R, 1024, 0, (cudaStream_t)stream>>>(logits, ld, V, nullptr, nullptr, 0, 0, nullptr, temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps,
+                                                                      (long long)eos_id, (long long)pad_id, finished, (long long*)tokens, (long long*)next_ids,
+                                                                      nullptr, 0, nullptr, Proc{});
     BR_CHECK_LAUNCH();
     return BR_OK;
 }
@@ -556,9 +642,9 @@ int br_sample_next_logp(const float* logits, int64_t ld, int R, int V, float tem
     if (do_sample) {
         BR_CHECK_ARG(temperature > 0.f && top_k >= 1 && top_k <= MAXC && top_p > 0.f && uniforms, "sample_next_logp: need T > 0, 1 <= top_k <= %d, top_p > 0 and a uniforms buffer", MAXC);
     }
-    sampler_kernel<true><<<R, 1024, 0, (cudaStream_t)stream>>>(logits, ld, V, nullptr, nullptr, 0, 0, nullptr, temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps,
-                                                              (long long)eos_id, (long long)pad_id, finished, (long long*)tokens, (long long*)next_ids,
-                                                              nullptr, 0, logp);
+    sampler_kernel<true, false><<<R, 1024, 0, (cudaStream_t)stream>>>(logits, ld, V, nullptr, nullptr, 0, 0, nullptr, temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps,
+                                                                     (long long)eos_id, (long long)pad_id, finished, (long long*)tokens, (long long*)next_ids,
+                                                                     nullptr, 0, logp, Proc{});
     BR_CHECK_LAUNCH();
     return BR_OK;
 }
@@ -576,9 +662,12 @@ int64_t br_sample_logp_workspace_bytes(int R, int V) {
     return br_sample_workspace_bytes(R, V) + (int64_t)R * n_chunks * sizeof(float2);
 }
 
+}  // extern "C"
+
+template <bool PROC>
 static int sample_2stage(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
                          const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id, int32_t* finished,
-                         int64_t* tokens, int64_t* next_ids, float* logp, void* workspace, void* stream) {
+                         int64_t* tokens, int64_t* next_ids, float* logp, void* workspace, void* stream, Proc pr = Proc{}) {
     BR_CHECK_ARG(R > 0 && V > 0 && workspace, "sample_next_2stage: empty / no workspace");
     const int k = do_sample ? top_k : 1;
     BR_CHECK_ARG(k >= 1 && k <= CAND_CAP / 2, "sample_next_2stage: top_k must be in [1, %d]", CAND_CAP / 2);
@@ -590,38 +679,84 @@ static int sample_2stage(const float* logits, int64_t ld, int R, int V, float te
     int* flags = ci + (int64_t)R * n_chunks * CAND_CAP;
     const int n_cand = n_chunks * CAND_CAP;
     if (!logp) {
-        BR_CHECK_CUDA(br_launch_pdl(sampler_partial_kernel<false>, dim3(n_chunks, R), dim3(256), 0, st, logits, (long long)ld, V, k, cv, ci, n_chunks,
-                                    flags, (float2*)nullptr));
-        BR_CHECK_CUDA(br_launch_pdl(sampler_kernel<false>, dim3(R), dim3(1024), 0, st, (const float*)cv, (long long)n_cand, n_cand, (const int*)ci,
+        BR_CHECK_CUDA(br_launch_pdl(sampler_partial_kernel<false, PROC>, dim3(n_chunks, R), dim3(256), 0, st, logits, (long long)ld, V, k, cv, ci, n_chunks,
+                                    flags, (float2*)nullptr, pr));
+        BR_CHECK_CUDA(br_launch_pdl(sampler_kernel<false, PROC>, dim3(R), dim3(1024), 0, st, (const float*)cv, (long long)n_cand, n_cand, (const int*)ci,
                                     logits, (long long)ld, V, (const int*)flags,
                                     temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps, (long long)eos_id, (long long)pad_id,
-                                    finished, (long long*)tokens, (long long*)next_ids, (const float2*)nullptr, n_chunks, (float*)nullptr));
+                                    finished, (long long*)tokens, (long long*)next_ids, (const float2*)nullptr, n_chunks, (float*)nullptr, pr));
         return BR_OK;
     }
     float2* stats = (float2*)(flags + flag_ints(R, n_chunks));             // the tail of br_sample_logp_workspace_bytes
-    BR_CHECK_CUDA(br_launch_pdl(sampler_partial_kernel<true>, dim3(n_chunks, R), dim3(256), 0, st, logits, (long long)ld, V, k, cv, ci, n_chunks,
-                                flags, stats));
-    BR_CHECK_CUDA(br_launch_pdl(sampler_kernel<true>, dim3(R), dim3(1024), 0, st, (const float*)cv, (long long)n_cand, n_cand, (const int*)ci,
+    BR_CHECK_CUDA(br_launch_pdl(sampler_partial_kernel<true, PROC>, dim3(n_chunks, R), dim3(256), 0, st, logits, (long long)ld, V, k, cv, ci, n_chunks,
+                                flags, stats, pr));
+    BR_CHECK_CUDA(br_launch_pdl(sampler_kernel<true, PROC>, dim3(R), dim3(1024), 0, st, (const float*)cv, (long long)n_cand, n_cand, (const int*)ci,
                                 logits, (long long)ld, V, (const int*)flags,
                                 temperature, top_k, top_p, do_sample, uniforms, step, R, max_steps, (long long)eos_id, (long long)pad_id,
-                                finished, (long long*)tokens, (long long*)next_ids, (const float2*)stats, n_chunks, logp));
+                                finished, (long long*)tokens, (long long*)next_ids, (const float2*)stats, n_chunks, logp, pr));
     return BR_OK;
 }
+
+extern "C" {
 
 /* two-stage variant for large vocabularies (same semantics as br_sample_next) */
 int br_sample_next_2stage(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
                           const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id, int32_t* finished,
                           int64_t* tokens, int64_t* next_ids, void* workspace, void* stream) {
-    return sample_2stage(logits, ld, R, V, temperature, top_k, top_p, do_sample, uniforms, step, max_steps, eos_id, pad_id, finished, tokens,
-                         next_ids, nullptr, workspace, stream);
+    return sample_2stage<false>(logits, ld, R, V, temperature, top_k, top_p, do_sample, uniforms, step, max_steps, eos_id, pad_id, finished, tokens,
+                                next_ids, nullptr, workspace, stream);
 }
 
 int br_sample_next_2stage_logp(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
                                const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id, int32_t* finished,
                                int64_t* tokens, int64_t* next_ids, float* logp, void* workspace, void* stream) {
     BR_CHECK_ARG(logp, "sample_next_2stage_logp: no logp buffer");
-    return sample_2stage(logits, ld, R, V, temperature, top_k, top_p, do_sample, uniforms, step, max_steps, eos_id, pad_id, finished, tokens,
-                         next_ids, logp, workspace, stream);
+    return sample_2stage<false>(logits, ld, R, V, temperature, top_k, top_p, do_sample, uniforms, step, max_steps, eos_id, pad_id, finished, tokens,
+                                next_ids, logp, workspace, stream);
+}
+
+// the processed entry points' arguments as the kernels take them; refuses what HF's processors refuse
+static int proc_args(const br_sample_proc* proc, int64_t eos_id, const int32_t* step, const char* what, Proc* out) {
+    BR_CHECK_ARG(proc, "%s: no br_sample_proc", what);
+    BR_CHECK_ARG(proc->repetition_penalty > 0.f, "%s: repetition_penalty must be > 0", what);
+    BR_CHECK_ARG(proc->min_p >= 0.f && proc->min_p <= 1.f, "%s: min_p must be in [0, 1]", what);
+    BR_CHECK_ARG(proc->min_new_tokens >= 0, "%s: min_new_tokens must be >= 0", what);
+    BR_CHECK_ARG(proc->repetition_penalty == 1.f || proc->presence, "%s: repetition_penalty != 1 needs a presence bitmap", what);
+    *out = Proc{proc->presence, proc->repetition_penalty, proc->min_p, proc->min_new_tokens, (long long)eos_id, step};
+    return BR_OK;
+}
+
+int br_sample_next_proc(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
+                        const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id, int32_t* finished,
+                        int64_t* tokens, int64_t* next_ids, float* logp, const br_sample_proc* proc, void* stream) {
+    BR_CHECK_ARG(R > 0 && V > 0, "sample_next_proc: empty");
+    if (do_sample) {
+        BR_CHECK_ARG(temperature > 0.f && top_k >= 1 && top_k <= MAXC && top_p > 0.f && uniforms, "sample_next_proc: need T > 0, 1 <= top_k <= %d, top_p > 0 and a uniforms buffer", MAXC);
+    }
+    Proc pr;
+    const int rc = proc_args(proc, eos_id, step, "sample_next_proc", &pr);
+    if (rc != BR_OK) return rc;
+    if (logp) {
+        sampler_kernel<true, true><<<R, 1024, 0, (cudaStream_t)stream>>>(logits, ld, V, nullptr, nullptr, 0, 0, nullptr, temperature, top_k, top_p, do_sample, uniforms, step, R,
+                                                                        max_steps, (long long)eos_id, (long long)pad_id, finished, (long long*)tokens,
+                                                                        (long long*)next_ids, nullptr, 0, logp, pr);
+    } else {
+        sampler_kernel<false, true><<<R, 1024, 0, (cudaStream_t)stream>>>(logits, ld, V, nullptr, nullptr, 0, 0, nullptr, temperature, top_k, top_p, do_sample, uniforms, step, R,
+                                                                         max_steps, (long long)eos_id, (long long)pad_id, finished, (long long*)tokens,
+                                                                         (long long*)next_ids, nullptr, 0, nullptr, pr);
+    }
+    BR_CHECK_LAUNCH();
+    return BR_OK;
+}
+
+int br_sample_next_2stage_proc(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
+                               const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id, int32_t* finished,
+                               int64_t* tokens, int64_t* next_ids, float* logp, const br_sample_proc* proc, void* workspace, void* stream) {
+    Proc pr;
+    const int rc = proc_args(proc, eos_id, step, "sample_next_2stage_proc", &pr);
+    if (rc != BR_OK) return rc;
+    return sample_2stage<true>(logits, ld, R, V, temperature, top_k, top_p, do_sample, uniforms, step, max_steps, eos_id, pad_id, finished, tokens,
+                               next_ids, logp, workspace, stream, pr);
 }
 
 int br_decode_advance(int32_t* step, int32_t* cur_len, int R, void* stream) {

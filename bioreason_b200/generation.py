@@ -2,7 +2,8 @@
 
 Replaces `DNALLMModel.generate` -> `text_model.generate(inputs_embeds=..., use_cache=True, **kw)` (dna_llm.py:246-305; HF
 generation/utils.py:2760-2800).  Semantics kept: completion-only ids; position_ids = cumsum(mask)-1 (pads excluded);
-warper order temperature -> top-k -> top-p; finished rows emit pad; output trimmed to the longest unfinished row.
+processor order repetition penalty -> min new tokens -> temperature -> top-k -> top-p -> min-p (the
+penalty set holds the generated tokens only, as with inputs_embeds); finished rows emit pad; output trimmed to the longest unfinished row.
 Redundancy removed (SURVEY.md §3.3): identical consecutive prompts (the G samples of a GRPO group) are encoded and
 prefilled once and share their prompt KV pages.
 """
@@ -22,6 +23,43 @@ from .packing import DecoderW
 PAGE = 64
 
 
+# HF generate() arguments that cannot change the ids or the return type: accepted and ignored.  Every other GenerationConfig field that
+# SamplingParams does not build is refused when it differs from HF's neutral value (_unbuilt_generation_args).
+_NO_EFFECT_ARGS = frozenset({
+    "use_cache", "cache_implementation", "cache_config", "compile_config", "disable_compile", "prefill_chunk_size", "low_memory",
+    "continuous_batching_config", "bos_token_id", "decoder_start_token_id", "is_assistant", "transformers_version", "_from_model_config",
+    "_commit_hash", "early_stopping", "length_penalty",          # beam search only (num_beams > 1 is refused)
+    "output_attentions", "output_hidden_states",                 # only with return_dict_in_generate (refused)
+    "num_assistant_tokens", "num_assistant_tokens_schedule", "assistant_confidence_threshold", "assistant_lookbehind",
+    "target_lookbehind", "assistant_early_exit",                 # only with an assistant model (refused)
+    "synced_gpus",
+})
+_BUILT_ARGS = frozenset({"max_new_tokens", "do_sample", "temperature", "top_k", "top_p", "eos_token_id", "pad_token_id",
+                         "repetition_penalty", "min_p", "min_new_tokens", "min_length", "max_length", "num_return_sequences"})
+# generate() arguments that are not GenerationConfig fields; refused unless None / empty
+_CALL_ARGS = ("logits_processor", "stopping_criteria", "prefix_allowed_tokens_fn", "assistant_model", "streamer", "negative_prompt_ids",
+              "negative_prompt_attention_mask", "custom_generate", "assistant_tokenizer", "tokenizer")
+
+
+def _unbuilt_generation_args(kwargs, gc):
+    """Names of the HF generation arguments set to a non-neutral value that the rollout does not implement (sorted).  Neutral = HF's
+    default (GenerationConfig._get_default_generation_params(), else None), so a bare GenerationConfig passes."""
+    from transformers import GenerationConfig
+    neutral = GenerationConfig._get_default_generation_params()
+    fields = set(GenerationConfig().to_dict()) | set(neutral)
+    bad = set()
+    for name in fields - _BUILT_ARGS - _NO_EFFECT_ARGS:
+        for src in (kwargs, vars(gc) if gc is not None else {}):
+            v = src.get(name, None)
+            if v is not None and v != neutral.get(name, None):
+                bad.add(name)
+    for name in _CALL_ARGS:
+        v = kwargs.get(name, None)
+        if v is not None and not (isinstance(v, (list, tuple)) and len(v) == 0):
+            bad.add(name)
+    return sorted(bad)
+
+
 @dataclass
 class SamplingParams:
     max_new_tokens: int = 20
@@ -31,10 +69,22 @@ class SamplingParams:
     top_p: float = 1.0
     eos_token_id: Optional[int] = None
     pad_token_id: Optional[int] = None
+    # HF logits processors, in HF's order: repetition penalty -> min new tokens (EOS blocked while fewer generated) -> (sampling only)
+    # temperature -> top-k -> top-p -> min-p
+    repetition_penalty: float = 1.0
+    min_p: float = 0.0
+    min_new_tokens: int = 0
+    num_return_sequences: int = 1       # DNALLMModel.generate repeats each row this many times before the rollout
 
     @classmethod
-    def from_hf_kwargs(cls, model_cfg, kwargs):
+    def from_hf_kwargs(cls, model_cfg, kwargs, prompt_width: Optional[int] = None):
+        """prompt_width: the padded prompt width P (HF's inputs_embeds width), which lowers min_length / max_length to new-token counts."""
         gc = kwargs.get("generation_config", None)
+        bad = _unbuilt_generation_args(kwargs, gc)
+        if bad:
+            raise NotImplementedError(f"generate(): {', '.join(bad)} not supported by the rollout (only max_new_tokens, do_sample, temperature, "
+                                      "top_k, top_p, min_p, repetition_penalty, min_new_tokens / min_length, num_return_sequences, "
+                                      "eos_token_id and pad_token_id are implemented)")
         def pick(name, default):
             if name in kwargs and kwargs[name] is not None:
                 return kwargs[name]
@@ -52,9 +102,60 @@ class SamplingParams:
         pad = pick("pad_token_id", getattr(model_cfg, "pad_token_id", None))
         if pad is None:
             pad = eos if eos is not None else 0
-        return cls(max_new_tokens=int(pick("max_new_tokens", 20)), do_sample=bool(pick("do_sample", False)),
+        max_new = pick("max_new_tokens", None)
+        if max_new is None and pick("max_length", None) is not None:
+            # HF then generates max_length - P tokens (inputs_embeds); not built
+            raise NotImplementedError("generate(): max_length without max_new_tokens is not supported by the rollout; pass max_new_tokens")
+        theta = float(pick("repetition_penalty", 1.0))
+        if not theta > 0:
+            raise ValueError(f"generate(): repetition_penalty must be a strictly positive float, got {theta}")
+        min_p = float(pick("min_p", 0.0))
+        if not 0.0 <= min_p <= 1.0:
+            raise ValueError(f"generate(): min_p must be in [0, 1], got {min_p}")
+        # HF _prepare_generated_length: min_new_tokens wins; else min_length lowered by the inputs_embeds width (the processors' input_ids
+        # hold only generated tokens)
+        m = pick("min_new_tokens", None)
+        if m is None:
+            ml = int(pick("min_length", 0))
+            if ml < 0:
+                raise ValueError(f"generate(): min_length must be >= 0, got {ml}")
+            if ml > 0 and prompt_width is None:
+                raise ValueError("generate(): min_length needs the prompt width")
+            m = max(ml - int(prompt_width or 0), 0)
+        m = int(m)
+        if m < 0:
+            raise ValueError(f"generate(): min_new_tokens must be >= 0, got {m}")
+        n = int(pick("num_return_sequences", 1))
+        if n < 1:
+            raise ValueError(f"generate(): num_return_sequences must be >= 1, got {n}")
+        do_sample = bool(pick("do_sample", False))
+        if n > 1 and not do_sample:
+            raise ValueError(f"generate(): greedy decoding does not support num_return_sequences = {n} (as in HF); pass do_sample=True")
+        return cls(max_new_tokens=int(max_new if max_new is not None else 20), do_sample=do_sample,
                    temperature=float(pick("temperature", 1.0)), top_k=int(pick("top_k", 50) or 0), top_p=float(pick("top_p", 1.0)),
-                   eos_token_id=eos, pad_token_id=pad)
+                   eos_token_id=eos, pad_token_id=pad, repetition_penalty=theta, min_p=min_p, min_new_tokens=m, num_return_sequences=n)
+
+
+def expand_return_sequences(input_ids, attention_mask, dna_tokenized, batch_idx_map, n: int):
+    """HF num_return_sequences: each row repeated n times in place (row b -> rows b n .. b n + n - 1), its DNA sequences with it.
+    Returns (input_ids, attention_mask, dna_tokenized, batch_idx_map); the DNA stays ordered by the new row index."""
+    if n == 1:
+        return input_ids, attention_mask, dna_tokenized, batch_idx_map
+    input_ids = input_ids.repeat_interleave(n, dim=0)
+    attention_mask = attention_mask.repeat_interleave(n, dim=0)
+    if dna_tokenized is not None and batch_idx_map:
+        order, new_map = [], []
+        for b in sorted(set(batch_idx_map)):
+            mine = [i for i, x in enumerate(batch_idx_map) if x == b]
+            for c in range(n):
+                order += mine
+                new_map += [b * n + c] * len(mine)
+        idx = torch.tensor(order, dtype=torch.long)
+        n_seq = len(batch_idx_map)
+        dna_tokenized = {k: (v[idx.to(v.device)] if torch.is_tensor(v) and v.dim() > 0 and v.shape[0] == n_seq else v)
+                         for k, v in dna_tokenized.items()}
+        batch_idx_map = new_map
+    return input_ids, attention_mask, dna_tokenized, batch_idx_map
 
 
 def detect_group_size(input_ids: torch.Tensor, dna_tokenized, batch_idx_map) -> torch.Tensor:
@@ -207,8 +308,12 @@ class RolloutEngine:
         nl = len(W.layers)
         # Static buffers + the captured decode graph are cached per rollout shape: a training run replays the same graph every
         # step (no per-step capture, no graph-pool / allocator churn -- that churn showed up as multi-second host stalls).
+        # the logits processors are baked into the captured sampler launch: they belong to the key
+        rep_pen = params.repetition_penalty
+        min_p = params.min_p if params.do_sample else 0.0                   # HF applies min-p only when sampling
+        min_new = params.min_new_tokens
         key = (B, G, tuple(plen), C, n_shared, max_pages, n_pages, params.do_sample, params.temperature, params.top_k, params.top_p,
-               params.eos_token_id, params.pad_token_id, id(Wd), bool(use_graph), bool(return_logprobs))
+               params.eos_token_id, params.pad_token_id, id(Wd), bool(use_graph), bool(return_logprobs), rep_pen, min_p, min_new)
         St = self._cached.get(key)
         hit = St is not None
         if not hit:
@@ -267,6 +372,8 @@ class RolloutEngine:
             St.ssq_b = torch.zeros(n_part_, 32, device=dev, dtype=torch.float32)    # ... entering the MLP (see br_skinny_gemm)
             St.ssq_e = torch.zeros(1, 32, device=dev, dtype=torch.float32)          # ... of the embedding row (first layer)
             St.samp_ws = ops.sample_workspace(R, cfg.vocab_size, dev, logp=return_logprobs)
+            # emitted-token bitmap of the repetition penalty (HF with inputs_embeds: only generated tokens count, not the prompt)
+            St.presence = ops.presence_bitmap(R, cfg.vocab_size, dev) if rep_pen != 1.0 else None
             St.graph = None
         else:
             St.tokens.fill_(pad_fill); St.finished.zero_(); St.step.zero_(); St.cur_len.copy_(cur0)
@@ -274,8 +381,12 @@ class RolloutEngine:
                 St.logp.zero_()
             if params.do_sample:
                 St.uniforms.copy_(uniforms)
+            if St.presence is not None:
+                St.presence.zero_()                                         # outside the graph, before the first token
         tokens, next_ids, finished, step, cur_len = St.tokens, St.next_ids, St.finished, St.step, St.cur_len
-        logp_kw = dict(logp=St.logp) if return_logprobs else {}
+        samp_kw = dict(logp=St.logp) if return_logprobs else {}
+        if rep_pen != 1.0 or min_p > 0.0 or min_new > 0:
+            samp_kw.update(repetition_penalty=rep_pen, min_p=min_p, min_new_tokens=min_new, presence=St.presence)
         uniforms = St.uniforms
         scratch, ws, attn_out, rope, h = St.scratch, St.ws, St.attn_out, St.rope, St.h
         ssq_a, ssq_b, ssq_e, samp_ws = St.ssq_a, St.ssq_b, St.ssq_e, St.samp_ws
@@ -286,7 +397,7 @@ class RolloutEngine:
             ops.sample_next(logits, workspace=samp_ws, temperature=params.temperature, top_k=params.top_k, top_p=params.top_p, do_sample=params.do_sample,
                             uniforms=uniforms if params.do_sample else None, step=step, max_steps=C, eos_id=eos,
                             pad_id=params.pad_token_id if params.pad_token_id is not None else 0, finished=finished, tokens=tokens,
-                            next_ids=next_ids, **logp_kw)
+                            next_ids=next_ids, **samp_kw)
 
         # ---- first token from the prefill's last position (row u replicated G times)
         last_rows = torch.tensor([u * P + P - 1 for u in range(U) for _ in range(G)], device=dev, dtype=torch.int32)
@@ -326,11 +437,12 @@ class RolloutEngine:
                 # warm up once on a side stream (allocator + lazy func attributes), then capture one decode step
                 s = torch.cuda.Stream()
                 s.wait_stream(torch.cuda.current_stream())
-                state = [t.clone() for t in (tokens, next_ids, finished, step, cur_len)]
+                live = tuple(t for t in (tokens, next_ids, finished, step, cur_len, St.presence) if t is not None)
+                state = [t.clone() for t in live]
                 with torch.cuda.stream(s):
                     decode_step()
                 torch.cuda.current_stream().wait_stream(s)
-                for t, v in zip((tokens, next_ids, finished, step, cur_len), state):
+                for t, v in zip(live, state):
                     t.copy_(v)                                                # the warm-up step is replayed for real below
                 St.graph = torch.cuda.CUDAGraph()
                 n0 = ops.LAUNCHES[0]
@@ -347,7 +459,7 @@ class RolloutEngine:
                         gc.enable()
                 St.per_replay = ops.LAUNCHES[0] - n0
                 ops.LAUNCHES[0] = n0
-                for t, v in zip((tokens, next_ids, finished, step, cur_len), state):
+                for t, v in zip(live, state):
                     t.copy_(v)
             self._cached[key] = St
         graph, per_replay, decode_step = St.graph, St.per_replay, St.decode_step

@@ -409,19 +409,24 @@ class DNALLMModel(nn.Module):
     @torch.no_grad()
     def generate(self, input_ids=None, attention_mask=None, dna_tokenized=None, batch_idx_map=None, **generation_kwargs):
         """dna_llm.py:246-305: completion-only ids.  Accepts loose kwargs (max_new_tokens, temperature, top_p, top_k,
-        do_sample; train_dna_qwen.py:279-289) and `generation_config=` (grpo_trainer.py:581-584).  Extra: `uniforms=`
-        [max_new_tokens, B] for replayable sampling; `return_logprobs=True` returns (ids, logps) (and stats last with `return_stats`),
+        do_sample; train_dna_qwen.py:279-289; repetition_penalty, min_p, min_new_tokens / min_length, num_return_sequences) and
+        `generation_config=` (grpo_trainer.py:581-584); loose kwargs win.  A non-default value of any other HF generation argument that
+        could change the ids or the return type raises NotImplementedError.  Extra: `uniforms=` [max_new_tokens, B * num_return_sequences]
+        for replayable sampling; `return_logprobs=True` returns (ids, logps) (and stats last with `return_stats`),
         logps [B, len] fp32 = each sampled token's log-prob under the rollout's raw logits (T = 1, full vocabulary), 0 after EOS."""
         if input_ids is None or attention_mask is None:
             raise ValueError("Either 'inputs' or 'input_ids'/'attention_mask' must be provided")
-        from ..generation import RolloutEngine, SamplingParams
+        from ..generation import RolloutEngine, SamplingParams, expand_return_sequences
         if getattr(self, "_rollout", None) is None:
             self._rollout = RolloutEngine(self)
         uniforms = generation_kwargs.pop("uniforms", None)
         use_graph = generation_kwargs.pop("use_graph", True)
         return_stats = generation_kwargs.pop("return_stats", False)
         return_logprobs = generation_kwargs.pop("return_logprobs", False)
-        params = SamplingParams.from_hf_kwargs(self.text_config, generation_kwargs)
+        params = SamplingParams.from_hf_kwargs(self.text_config, generation_kwargs, prompt_width=input_ids.shape[1])
+        # num_return_sequences: n consecutive copies of each row (HF's expansion); the engine's group detection prefills each prompt once
+        input_ids, attention_mask, dna_tokenized, batch_idx_map = expand_return_sequences(input_ids, attention_mask, dna_tokenized,
+                                                                                          batch_idx_map, params.num_return_sequences)
         return self._rollout.generate(input_ids, attention_mask, dna_tokenized, batch_idx_map, params=params, uniforms=uniforms,
                                       use_graph=use_graph, return_stats=return_stats, return_logprobs=return_logprobs)
 

@@ -414,10 +414,18 @@ def sample_workspace(R, V, device, logp: bool = False):
 
 
 def sample_next(logits, *, temperature=1.0, top_k=20, top_p=1.0, do_sample=True, uniforms=None, step=None, max_steps=1,
-                eos_id=-1, pad_id=0, finished=None, tokens=None, next_ids=None, workspace=None, logp=None):
-    """logp: optional fp32 [R, max_steps]; receives log_softmax(logits)[r, token] at column step (0 for finished rows)."""
+                eos_id=-1, pad_id=0, finished=None, tokens=None, next_ids=None, workspace=None, logp=None,
+                repetition_penalty=1.0, min_p=0.0, min_new_tokens=0, presence=None):
+    """logp: optional fp32 [R, max_steps]; receives log_softmax(logits)[r, token] at column step (0 for finished rows).
+    repetition_penalty / min_new_tokens / min_p: HF's logits processors (br_sample_next*_proc).  presence: int32 [R, ceil(V / 32)] bitmap
+    of the tokens each row has emitted (zeroed by the caller before the first draw, updated by every call), needed when
+    repetition_penalty != 1.  With all three at their defaults the launches are those of the sampler without processors."""
     R, V = logits.shape
     assert logits.dtype == torch.float32
+    if repetition_penalty != 1.0 or min_p != 0.0 or min_new_tokens != 0:
+        _sample_next_proc(logits, R, V, temperature, top_k, top_p, do_sample, uniforms, step, max_steps, eos_id, pad_id, finished, tokens,
+                          next_ids, workspace, logp, repetition_penalty, min_p, min_new_tokens, presence)
+        return
     if logp is not None:
         _sample_next_logp(logits, R, V, temperature, top_k, top_p, do_sample, uniforms, step, max_steps, eos_id, pad_id, finished, tokens,
                           next_ids, workspace, logp)
@@ -449,6 +457,38 @@ def _sample_next_logp(logits, R, V, temperature, top_k, top_p, do_sample, unifor
                                     1 if do_sample else 0, ptr(uniforms, "float*"), ptr(step, "int32_t*"), int(max_steps), int(eos_id),
                                     int(pad_id), ptr(finished, "int32_t*"), ptr(tokens, "int64_t*"), ptr(next_ids, "int64_t*"),
                                     ptr(logp, "float*"), _stream()), "sample_next_logp")
+
+
+def presence_bitmap(R, V, device):
+    """The processed sampler's emitted-token bitmap: int32 [R, ceil(V / 32)], zeroed."""
+    return torch.zeros(R, (V + 31) // 32, device=device, dtype=torch.int32)
+
+
+def _sample_next_proc(logits, R, V, temperature, top_k, top_p, do_sample, uniforms, step, max_steps, eos_id, pad_id, finished, tokens,
+                      next_ids, workspace, logp, repetition_penalty, min_p, min_new_tokens, presence):
+    _need_cuda(logits, logp, presence)
+    if presence is not None:
+        assert presence.dtype == torch.int32 and presence.is_contiguous() and presence.shape == (R, (V + 31) // 32), \
+            ("presence must be int32 [R, ceil(V / 32)] contiguous", tuple(presence.shape), R, V)
+    if logp is not None:
+        assert logp.dtype == torch.float32 and logp.is_contiguous() and logp.shape == (R, max_steps), (logp.shape, R, max_steps)
+    proc = ffi.new("br_sample_proc*")
+    proc.repetition_penalty = float(repetition_penalty)
+    proc.min_p = float(min_p)
+    proc.min_new_tokens = int(min_new_tokens)
+    proc.presence = ptr(presence, "uint32_t*")
+    if workspace is not None and (not do_sample or top_k <= 32):
+        if logp is not None:
+            assert workspace.numel() >= lib().br_sample_logp_workspace_bytes(R, V), "logp needs sample_workspace(R, V, device, logp=True)"
+        check(lib().br_sample_next_2stage_proc(ptr(logits, "float*"), _row_major_2d(logits), R, V, float(temperature), int(top_k), float(top_p),
+                                               1 if do_sample else 0, ptr(uniforms, "float*"), ptr(step, "int32_t*"), int(max_steps), int(eos_id),
+                                               int(pad_id), ptr(finished, "int32_t*"), ptr(tokens, "int64_t*"), ptr(next_ids, "int64_t*"),
+                                               ptr(logp, "float*"), proc, ptr(workspace), _stream()), "sample_next_2stage_proc")
+        return
+    check(lib().br_sample_next_proc(ptr(logits, "float*"), _row_major_2d(logits), R, V, float(temperature), int(top_k), float(top_p),
+                                    1 if do_sample else 0, ptr(uniforms, "float*"), ptr(step, "int32_t*"), int(max_steps), int(eos_id),
+                                    int(pad_id), ptr(finished, "int32_t*"), ptr(tokens, "int64_t*"), ptr(next_ids, "int64_t*"),
+                                    ptr(logp, "float*"), proc, _stream()), "sample_next_proc")
 
 
 def decode_advance(step, cur_len):

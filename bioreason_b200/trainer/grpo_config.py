@@ -76,6 +76,8 @@ class DNALLMGRPOConfig:
     fp8_rollout: bool = False             # rollout decode streams e4m3 layer weights (per-row scales); samples from the quantized policy
     rollout_is_correction: bool = False   # weight each token's policy-gradient term by min(exp(old - rollout logp), rollout_is_cap)
     rollout_is_cap: float = 2.0           # truncation of that importance weight (> 0; inf: untruncated)
+    sampling_from_config: bool = False    # rollout takes temperature / top_p / top_k / min_p / repetition_penalty from this config (later
+                                          # TRL releases); off: the reference's hard-coded T = 0.6, top_p = 0.95, top_k = 20
 
     def __post_init__(self):
         if not (self.rollout_is_cap > 0):

@@ -130,6 +130,10 @@ class DNALLMGRPOTrainer:
         # hard-coded exactly like grpo_trainer.py:384-391 (args.temperature/top_p/top_k are NOT consulted there either)
         self.generation_kwargs = dict(max_new_tokens=self.max_completion_length, do_sample=True, temperature=0.6, top_p=0.95, top_k=20,
                                       pad_token_id=self.pad_token_id, eos_token_id=None if a.suppress_eos else self.eos_token_id)
+        if getattr(a, "sampling_from_config", False):
+            # later TRL releases read the sampling fields of the config (min_p None: off, as in HF)
+            self.generation_kwargs.update(temperature=a.temperature, top_p=a.top_p, top_k=a.top_k, min_p=a.min_p,
+                                          repetition_penalty=a.repetition_penalty)
         if getattr(a, "rollout_is_correction", False):
             # the sampler's own log-probs of the tokens it drew (behaviour policy: merged / FP8 decode weights) for the IS weights
             self.generation_kwargs["return_logprobs"] = True

@@ -215,6 +215,30 @@ int br_sample_next_logp(const float* logits, int64_t ld, int R, int V, float tem
 int br_sample_next_2stage_logp(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
                                const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id,
                                int32_t* finished, int64_t* tokens, int64_t* next_ids, float* logp, void* workspace, void* stream);
+/* Logits processors of the processed samplers (HF generation/logits_process.py), applied in HF's order on the fp32 logits row z:
+ *   repetition penalty theta: z_j = z_j < 0 ? z_j * theta : z_j / theta (fp32, IEEE division) for each distinct token j whose bit is set
+ *     in presence[r] (bit j % 32 of word j / 32 of row r; the bitmap is [R, ceil(V / 32)] uint32, contiguous);
+ *   min_new_tokens m: z[eos_id] = -inf while *step < m (step NULL: 0; nothing when eos_id < 0);
+ *   then temperature -> top-k -> top-p as above, then min-p: drop every kept token with exp((z_j - z_max) / T) < min_p (the maximum
+ *     always stays).  Greedy (!do_sample) takes the argmax of the penalised, EOS-masked row; T, top-k, top-p and min_p do nothing there.
+ * After the draw each row sets the bit of the token it emits (pad for a finished row).  The caller zeroes presence before a sequence's
+ * first draw; presence may be NULL only when repetition_penalty == 1 (then nothing is penalised or recorded).  Refused: theta <= 0,
+ * min_p outside [0, 1], min_new_tokens < 0.  logp (NULL: none) is the behaviour log-prob of the *_logp entry points: the RAW logits
+ * (T = 1, full vocabulary, no processor) at the chosen token; the two-stage one then needs br_sample_logp_workspace_bytes.  With
+ * theta = 1, min_p = 0 and m = 0 the tokens and logp equal those of the entry points above. */
+typedef struct br_sample_proc {
+    float repetition_penalty;    /* theta > 0; 1: off */
+    float min_p;                 /* [0, 1]; 0: off */
+    int32_t min_new_tokens;      /* m >= 0; 0: off */
+    uint32_t* presence;          /* [R, ceil(V / 32)] emitted-token bitmap, read before and updated after the draw */
+} br_sample_proc;
+int br_sample_next_proc(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
+                        const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id, int32_t* finished,
+                        int64_t* tokens, int64_t* next_ids, float* logp, const br_sample_proc* proc, void* stream);
+int br_sample_next_2stage_proc(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,
+                               const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id,
+                               int32_t* finished, int64_t* tokens, int64_t* next_ids, float* logp, const br_sample_proc* proc,
+                               void* workspace, void* stream);
 int br_decode_advance(int32_t* step, int32_t* cur_len, int R, void* stream);
 
 /* Decode attention, one launch per layer per step: per-head q/k RMSNorm + RoPE at cur_len[r], K/V append to the row's page,
