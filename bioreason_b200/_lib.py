@@ -54,7 +54,7 @@ def last_error() -> str:
     return ffi.string(buf).decode()
 
 
-_KERNELS_PER_CALL = {"lmhead_logprob_fwd": 2, "attn_bwd": 2, "sample_next_2stage": 2, "sample_next_2stage_logp": 2,
+_KERNELS_PER_CALL = {"lmhead_logprob_fwd": 2, "lmhead_logprob_entropy_fwd": 2, "attn_bwd": 2, "sample_next_2stage": 2, "sample_next_2stage_logp": 2,
                      "sample_next_2stage_proc": 2,
                      "quantize_rows_e4m3": 2}
 COUNTER = [0]

@@ -14,7 +14,8 @@
 // accumulator, multiplied by that projection's counter-based mask and 1 / (1 - p_eff) in registers, and added to the main accumulator
 // before the usual epilogue (one rounding, no extra HBM traffic).
 // Epilogue modes: plain (+bias, +residual, gated-SiLU on interleaved column pairs, fp32/bf16 out, row scatter),
-// online log-sum-exp partials + target-logit gather (lm_head; logits never reach HBM), and softmax-gradient tiles.
+// online log-sum-exp partials + target-logit gather (lm_head; logits never reach HBM; optionally with entropy partials),
+// and softmax-gradient tiles.
 #include "br_common.cuh"
 #include "../../include/bioreason_b200.h"
 #include "lora_dropout.cuh"
@@ -26,7 +27,7 @@ constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int NTHREADS = 288;
 
-enum { MODE_STD = 0, MODE_LSE = 1, MODE_DLOGITS = 2 };
+enum { MODE_STD = 0, MODE_LSE = 1, MODE_DLOGITS = 2, MODE_LSE_ENT = 3 };   // MODE_LSE_ENT: MODE_LSE + the entropy partials
 
 struct GemmParams {
     int M, N, K, K2;
@@ -47,6 +48,7 @@ struct GemmParams {
                                    // (MODE_LSE writes one partial per 128-column tile: [M, n_tiles_n])
     int group_m;             // m-blocks per raster group (see tile_coords)
     br::DropParams drop;     // MASK: dropout of the second segment's projections
+    float* pent;             // MODE_LSE_ENT: [M, n_tiles_n] u_t = sum over the tile of exp(z - m_t) (z - m_t)  (<= 0)
 };
 
 template <int BN>
@@ -269,9 +271,10 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                     else *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.D) + orow * (long long)p.ldd + col) = br::pack_bf16(x0, x1);
                 }
             }
-        } else if constexpr (MODE == MODE_LSE) {
+        } else if constexpr (MODE == MODE_LSE || MODE == MODE_LSE_ENT) {
             // per-row max / sum-exp over each 128-column tile (the four lanes of a quad share a row) + target-logit pick.  A 256-wide
             // tile writes its two halves as two partials, so the partials and their combine do not depend on the tile width.
+            // MODE_LSE_ENT also sums exp(z - m) (z - m) from the same exps; every term is <= 0, so the partial keeps its sign.
 #pragma unroll
             for (int h = 0; h < NSUB; ++h) {
                 const int nh = n0 + 128 * h;
@@ -287,21 +290,33 @@ gemm_tc5_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                         if (nh + 8 * i < p.N) mx = fmaxf(mx, fmaxf(acc[64 * h + 4 * i + 2 * hh], acc[64 * h + 4 * i + 2 * hh + 1]) * p.alpha);
                     mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
                     mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-                    float sm = 0.f;
+                    float sm = 0.f, un = 0.f;
 #pragma unroll
                     for (int i = 0; i < 16; ++i) {
                         if (nh + 8 * i >= p.N) continue;
                         const int col = nh + 8 * i + cq;
                         const float x0 = acc[64 * h + 4 * i + 2 * hh] * p.alpha, x1 = acc[64 * h + 4 * i + 2 * hh + 1] * p.alpha;
-                        sm += __expf(x0 - mx) + __expf(x1 - mx);
+                        if constexpr (MODE == MODE_LSE_ENT) {
+                            const float d0 = x0 - mx, d1 = x1 - mx;
+                            const float e0 = __expf(d0), e1 = __expf(d1);
+                            sm += e0 + e1;
+                            un += e0 * d0 + e1 * d1;
+                        } else {
+                            sm += __expf(x0 - mx) + __expf(x1 - mx);
+                        }
                         if (col == tgt) p.tgt_logit[row] = x0;
                         if (col + 1 == tgt) p.tgt_logit[row] = x1;
                     }
                     sm += __shfl_xor_sync(0xffffffffu, sm, 1);
                     sm += __shfl_xor_sync(0xffffffffu, sm, 2);
+                    if constexpr (MODE == MODE_LSE_ENT) {
+                        un += __shfl_xor_sync(0xffffffffu, un, 1);
+                        un += __shfl_xor_sync(0xffffffffu, un, 2);
+                    }
                     if (row_ok && (lane & 3) == 0) {
                         p.pmax[(long long)row * p.n_tiles_n + nb * NSUB + h] = mx;
                         p.psum[(long long)row * p.n_tiles_n + nb * NSUB + h] = sm;
+                        if constexpr (MODE == MODE_LSE_ENT) p.pent[(long long)row * p.n_tiles_n + nb * NSUB + h] = un;
                     }
                 }
             }
@@ -345,6 +360,37 @@ __global__ void lse_combine_kernel(const float* __restrict__ pmax, const float* 
     }
 }
 
+// lse_combine_kernel plus the entropy H = -sum_j p_j log p_j of the row (p = softmax of the row's logits).  With M = max_t m_t and
+// r_t = exp(m_t - M):  S = sum_t s_t r_t,  U = sum_t r_t (u_t + (m_t - M) s_t),  H = log S - U / S.  S and lse are formed exactly as
+// lse_combine_kernel forms them (same loops, same order), so lse and logp are bit-identical to it.  Every term of U is <= 0 and
+// S >= 1 (the maximal tile contributes s_t >= exp(0) = 1), so both terms of H are >= 0 and H >= 0 in floating point as well.
+__global__ void lse_entropy_combine_kernel(const float* __restrict__ pmax, const float* __restrict__ psum, const float* __restrict__ pent,
+                                           const float* __restrict__ tgt_logit, const int* __restrict__ target, int M, int nt,
+                                           float* __restrict__ lse, float* __restrict__ logp, float* __restrict__ ent) {
+    int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= M) return;
+    int lane = threadIdx.x & 31;
+    float mx = -INFINITY;
+    for (int t = lane; t < nt; t += 32) mx = fmaxf(mx, pmax[(long long)row * nt + t]);
+    mx = br::warp_max(mx);
+    float s = 0.f, u = 0.f;
+    for (int t = lane; t < nt; t += 32) {
+        const float dm = pmax[(long long)row * nt + t] - mx;
+        const float r = __expf(dm), st = psum[(long long)row * nt + t];
+        s += st * r;
+        u += r * (pent[(long long)row * nt + t] + dm * st);
+    }
+    s = br::warp_sum(s);
+    u = br::warp_sum(u);
+    if (lane == 0) {
+        const float ls = logf(s);
+        float l = ls + mx;
+        if (lse) lse[row] = l;
+        if (logp) logp[row] = (target[row] >= 0) ? tgt_logit[row] - l : 0.f;
+        ent[row] = ls - u / s;
+    }
+}
+
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -379,6 +425,7 @@ int launch_mode(int mode, const CUtensorMap& a, const CUtensorMap& b, const CUte
                 cudaStream_t st) {
     if (mode == MODE_STD) return launch<BN, MODE_STD>(a, b, a2, b2, p, st);
     if (mode == MODE_LSE) return launch<BN, MODE_LSE>(a, b, a2, b2, p, st);
+    if (mode == MODE_LSE_ENT) return launch<BN, MODE_LSE_ENT>(a, b, a2, b2, p, st);
     return launch<BN, MODE_DLOGITS>(a, b, a2, b2, p, st);
 }
 
@@ -494,6 +541,33 @@ int br_lmhead_logprob_fwd(const void* H, int64_t ldh, const void* W, int64_t ldw
     if (rc) return rc;
     const int wpb = 8;
     lse_combine_kernel<<<(M + wpb - 1) / wpb, wpb * 32, 0, st>>>(p.pmax, p.psum, p.tgt_logit, target, M, p.n_tiles_n, lse, logp);
+    BR_CHECK_LAUNCH();
+    return BR_OK;
+}
+
+int64_t br_lmhead_entropy_workspace_bytes(int M, int V) {
+    int nt = (V + 127) / 128;   // (max, sum-exp, entropy) partials per 128-column tile
+    return (int64_t)M * nt * 3 * sizeof(float) + (int64_t)M * sizeof(float);
+}
+
+int br_lmhead_logprob_entropy_fwd(const void* H, int64_t ldh, const void* W, int64_t ldw, const int32_t* target, int M, int V, int K,
+                                  float scale, float* logp, float* lse, float* entropy, void* workspace, void* stream) {
+    BR_CHECK_ARG(entropy, "lmhead_logprob_entropy: needs entropy");
+    GemmParams p;
+    memset(&p, 0, sizeof(p));
+    int nt_max = (V + 127) / 128;
+    p.alpha = scale; p.target = target;
+    p.pmax = reinterpret_cast<float*>(workspace);
+    p.psum = p.pmax + (int64_t)M * nt_max;
+    p.pent = p.psum + (int64_t)M * nt_max;
+    p.tgt_logit = p.pent + (int64_t)M * nt_max;
+    cudaStream_t st = (cudaStream_t)stream;
+    BR_CHECK_CUDA(cudaMemsetAsync(p.tgt_logit, 0, (size_t)M * sizeof(float), st));
+    int rc = run_gemm(MODE_LSE_ENT, H, ldh, W, ldw, M, V, K, nullptr, 0, nullptr, 0, 0, p, st);
+    if (rc) return rc;
+    const int wpb = 8;
+    lse_entropy_combine_kernel<<<(M + wpb - 1) / wpb, wpb * 32, 0, st>>>(p.pmax, p.psum, p.pent, p.tgt_logit, target, M, p.n_tiles_n, lse,
+                                                                         logp, entropy);
     BR_CHECK_LAUNCH();
     return BR_OK;
 }

@@ -27,6 +27,30 @@ def gather_rewards(rewards_per_func: torch.Tensor) -> torch.Tensor:
     return torch.cat(parts, 0)
 
 
+def gather_masked(values: torch.Tensor, mask: torch.Tensor):
+    """All ranks' values and int32 masks, flattened and concatenated in rank order (for a statistic over the valid entries of the
+    whole batch, such as the entropy threshold).  Ranks may hold different numbers of entries (completion widths differ): each pads
+    to the largest with mask 0, so the padding is never valid.  One host sync for the sizes when world > 1."""
+    v = values.reshape(-1)
+    m = mask.reshape(-1).to(torch.int32)
+    rank, ws = world()
+    if ws == 1:
+        return v, m
+    n = torch.tensor([v.numel()], device=v.device, dtype=torch.int64)
+    sizes = [torch.empty_like(n) for _ in range(ws)]
+    dist.all_gather(sizes, n)
+    n_max = max(int(x.item()) for x in sizes)
+    vp = torch.zeros(n_max, device=v.device, dtype=v.dtype)
+    mp = torch.zeros(n_max, device=v.device, dtype=torch.int32)
+    vp[:v.numel()] = v
+    mp[:m.numel()] = m
+    parts_v = [torch.empty_like(vp) for _ in range(ws)]
+    parts_m = [torch.empty_like(mp) for _ in range(ws)]
+    dist.all_gather(parts_v, vp)
+    dist.all_gather(parts_m, mp)
+    return torch.cat(parts_v), torch.cat(parts_m)
+
+
 def local_slice(x: torch.Tensor, rows_local: int) -> torch.Tensor:
     """grpo_trainer.py:695-699."""
     rank, _ = world()

@@ -77,6 +77,45 @@ def grpo_loss_is_raw(lp, old_lp, ref_lp, rollout_lp, adv, mask, beta, eps_low, e
     return out3, stats, dlp
 
 
+def grpo_loss_ent_raw(lp, old_lp, ref_lp, rollout_lp, adv, mask, entropy, tau, beta, eps_low, eps_high, is_cap=2.0, want_grad=True):
+    """grpo_loss_raw (grpo_loss_is_raw when rollout_lp is given) with high-entropy token selection (br_grpo_loss_ent_fwd_bwd): a token's
+    policy-gradient term is kept only where mask and entropy >= tau (fp32 [1] on the device, entropy_threshold); the KL term is not
+    masked.  tau = -inf gives the plain (or IS) loss bit for bit.
+    Returns (out3, is_stats or None, ent_sum [1] = sum of mask * entropy, dlp)."""
+    _need_cuda(lp, adv, mask, entropy, tau)
+    B, C = lp.shape
+    lp = lp.float().contiguous()
+    old_lp = None if old_lp is None else old_lp.float().contiguous()
+    ref_lp = None if ref_lp is None else ref_lp.float().contiguous()
+    rollout_lp = None if rollout_lp is None else rollout_lp.float().contiguous()
+    entropy = entropy.float().contiguous()
+    assert entropy.shape == (B, C) and tau.dtype == torch.float32 and tau.numel() == 1, (entropy.shape, lp.shape, tau.dtype)
+    adv = adv.float().contiguous()
+    mask = mask.to(torch.int32).contiguous()
+    out3 = torch.empty(3, device=lp.device, dtype=torch.float32)
+    stats = torch.empty(4, device=lp.device, dtype=torch.float32) if rollout_lp is not None else None
+    ent_sum = torch.empty(1, device=lp.device, dtype=torch.float32)
+    dlp = torch.empty_like(lp) if want_grad else None
+    check(lib().br_grpo_loss_ent_fwd_bwd(ptr(lp, "float*"), ptr(old_lp, "float*"), ptr(ref_lp, "float*"), ptr(rollout_lp, "float*"),
+                                         ptr(adv, "float*"), ptr(mask, "int32_t*"), ptr(entropy, "float*"), ptr(tau, "float*"), B, C,
+                                         float(beta), float(eps_low), float(eps_high), float(is_cap), ptr(out3, "float*"),
+                                         ptr(stats, "float*"), ptr(ent_sum, "float*"), ptr(dlp, "float*"), _stream()), "grpo_loss_ent")
+    return out3, stats, ent_sum, dlp
+
+
+def entropy_threshold(entropy: torch.Tensor, mask: torch.Tensor, level: float) -> torch.Tensor:
+    """fp32 [1] on the device: torch.quantile(entropy[mask != 0].float(), level) bit for bit (+inf when no entry is valid), without a
+    host sync.  TRL's top_entropy_quantile rho takes level = 1 - rho."""
+    _need_cuda(entropy, mask)
+    x = entropy.reshape(-1).float().contiguous()
+    m = mask.reshape(-1).to(torch.int32).contiguous()
+    assert x.numel() == m.numel(), (x.shape, m.shape)
+    tau = torch.empty(1, device=x.device, dtype=torch.float32)
+    check(lib().br_entropy_threshold(ptr(x, "float*"), ptr(m, "int32_t*"), x.numel(), float(level), ptr(tau, "float*"), _stream()),
+          "entropy_threshold")
+    return tau
+
+
 class _GRPOLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, lp, old_lp, ref_lp, adv, mask, beta, eps_low, eps_high):
@@ -166,15 +205,23 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, bias=None, residual=None, alpha: f
     return out
 
 
-def lmhead_logprob(h: torch.Tensor, w: torch.Tensor, target: torch.Tensor, scale: float = 1.0):
-    """Fused lm_head + log_softmax + gather (grpo_trainer.py:511-520): returns (logp[M], lse[M]) fp32."""
+def lmhead_logprob(h: torch.Tensor, w: torch.Tensor, target: torch.Tensor, scale: float = 1.0, want_entropy: bool = False):
+    """Fused lm_head + log_softmax + gather (grpo_trainer.py:511-520): returns (logp[M], lse[M]) fp32.
+    want_entropy: also the entropy of every row's softmax, (logp, lse, entropy[M]); logp and lse are the same bits."""
     _need_cuda(h, w, target)
     M, K = h.shape
     V = w.shape[0]
     tgt = target.to(torch.int32).contiguous()
-    ws = torch.empty(lib().br_lmhead_workspace_bytes(M, V), device=h.device, dtype=torch.uint8)
     logp = torch.empty(M, device=h.device, dtype=torch.float32)
     lse = torch.empty(M, device=h.device, dtype=torch.float32)
+    if want_entropy:
+        ent = torch.empty(M, device=h.device, dtype=torch.float32)
+        ws = torch.empty(lib().br_lmhead_entropy_workspace_bytes(M, V), device=h.device, dtype=torch.uint8)
+        check(lib().br_lmhead_logprob_entropy_fwd(ptr(h), _row_major_2d(h), ptr(w), _row_major_2d(w), ptr(tgt, "int32_t*"), M, V, K,
+                                                  float(scale), ptr(logp, "float*"), ptr(lse, "float*"), ptr(ent, "float*"), ptr(ws),
+                                                  _stream()), "lmhead_logprob_entropy_fwd")
+        return logp, lse, ent
+    ws = torch.empty(lib().br_lmhead_workspace_bytes(M, V), device=h.device, dtype=torch.uint8)
     check(lib().br_lmhead_logprob_fwd(ptr(h), _row_major_2d(h), ptr(w), _row_major_2d(w), ptr(tgt, "int32_t*"), M, V, K,
                                       float(scale), ptr(logp, "float*"), ptr(lse, "float*"), ptr(ws), _stream()),
           "lmhead_logprob_fwd")

@@ -78,7 +78,12 @@ class DNALLMGRPOConfig:
     rollout_is_cap: float = 2.0           # truncation of that importance weight (> 0; inf: untruncated)
     sampling_from_config: bool = False    # rollout takes temperature / top_p / top_k / min_p / repetition_penalty from this config (later
                                           # TRL releases); off: the reference's hard-coded T = 0.6, top_p = 0.95, top_k = 20
+    top_entropy_quantile: float = 1.0     # keep the policy-gradient term on the top rho fraction of completion tokens by entropy, over
+                                          # all ranks per loss call (TRL; "Beyond the 80/20 Rule"); 1.0: off
+    log_entropy: bool = False             # log the policy's mean token entropy (`entropy`) without masking
 
     def __post_init__(self):
+        if not (0.0 <= self.top_entropy_quantile <= 1.0):
+            raise ValueError(f"top_entropy_quantile must lie in [0, 1] (1.0: off), got {self.top_entropy_quantile}")
         if not (self.rollout_is_cap > 0):
             raise ValueError(f"rollout_is_cap must be > 0 (inf for untruncated importance sampling), got {self.rollout_is_cap}")

@@ -223,6 +223,23 @@ class DNALLMGRPOTrainer:
                                             save=False, lora=lora, dropout=dropout, **({"group_size": group_size} if group_size else {}))
         return lp
 
+    def _get_per_token_logps_and_entropies(self, model, input_ids, attention_mask, keep_last, lora="policy", dropout=False, group_size=None,
+                                           dropout_pass=None, row_offset=0, **mm):
+        """No-grad (log-probs, entropies) [B, keep_last] of the fused lm-head pass (TRL's method of this name; T = 1).  dropout_pass /
+        row_offset as training.policy_forward takes them, so a row chunk reproduces the LoRA dropout masks of a whole pass."""
+        kw = dict(group_size=group_size) if group_size else {}
+        if dropout_pass is not None:
+            kw.update(dropout_pass=dropout_pass, row_offset=row_offset)
+        with torch.no_grad():
+            lp, _, ent = training.policy_forward(model, input_ids, attention_mask, mm.get("dna_tokenized"), mm.get("batch_idx_map"), keep_last,
+                                                 save=False, lora=lora, dropout=dropout, want_entropy=True, **kw)
+        return lp, ent
+
+    def _entropy_threshold(self, entropies, completion_mask, rho):
+        """Device fp32 [1]: TRL's threshold torch.quantile(valid entropies of all ranks, 1 - rho); +inf when no token is valid."""
+        vals, valid = dp.gather_masked(entropies, completion_mask)
+        return ops.entropy_threshold(vals, valid, 1.0 - rho)
+
     def _local_group_size(self, prompt_ids, mm) -> Optional[int]:
         """Rows per prompt group in this rank's rows when share_prompt_prefix is on (None when off): consecutive identical prompts
         (text and DNA), so a rank holding part of a group still shares it.  One host sync."""
@@ -350,6 +367,31 @@ class DNALLMGRPOTrainer:
             is_acc = torch.zeros(4, device=ids.device)
         # one LoRA-dropout pass for all row chunks; each chunk passes its first row so the masks ignore the chunking
         pid = model.new_lora_dropout_pass() if getattr(model, "_lora", None) is not None else None
+        # high-entropy token selection (TRL's top_entropy_quantile): one threshold per call over the valid completion tokens of all
+        # ranks.  It must not depend on the row chunking, so with several chunks a no-grad pre-pass (same dropout pass, same row
+        # offsets: the same entropies, checked below) scores every row first; with one chunk the loss pass's own entropies are used.
+        rho = float(getattr(self.args, "top_entropy_quantile", 1.0))
+        masking = rho < 1.0
+        want_ent = masking or bool(getattr(self.args, "log_entropy", False))
+        tau = pre_ent = ent_diff = None
+        if want_ent:
+            ent_acc = torch.zeros(1, device=ids.device)
+            if not masking:
+                tau = torch.full((1,), -float("inf"), device=ids.device)    # keeps every token: the loss of grpo_loss_raw, bit for bit
+            elif mr < B:
+                t0 = time.perf_counter()
+                with self._mark("entropy_prepass"):
+                    parts = []
+                    for lo in range(0, B, mr):
+                        hi = min(B, lo + mr)
+                        mm_c = _slice_mm(mm, lo, hi)
+                        parts.append(self._get_per_token_logps_and_entropies(
+                            model, ids[lo:hi], mask[lo:hi], C, dropout=pid is not None, group_size=gs, dropout_pass=pid, row_offset=lo,
+                            **mm_c)[1])
+                    pre_ent = torch.cat(parts)
+                    tau = self._entropy_threshold(pre_ent, completion_mask, rho)
+                    ent_diff = torch.zeros((), dtype=torch.bool, device=ids.device)
+                self.timings["entropy_prepass"] += time.perf_counter() - t0
         for lo in range(0, B, mr):
             hi = min(B, lo + mr)
             sl = slice(lo, hi)
@@ -357,9 +399,22 @@ class DNALLMGRPOTrainer:
             t0 = time.perf_counter()
             with self._mark("policy_fwd"):
                 drop_kw = dict(dropout=True, dropout_pass=pid, row_offset=lo) if pid is not None else {}
-                lp, ctx = training.policy_forward(model, ids[sl], mask[sl], mm_c["dna_tokenized"], mm_c["batch_idx_map"], C, save=backward,
-                                                  **({"group_size": gs} if gs else {}), **drop_kw)
-            if tis:
+                ent_kw = dict(want_entropy=True) if want_ent else {}
+                out = training.policy_forward(model, ids[sl], mask[sl], mm_c["dna_tokenized"], mm_c["batch_idx_map"], C, save=backward,
+                                              **({"group_size": gs} if gs else {}), **drop_kw, **ent_kw)
+                lp, ctx = out[0], out[1]
+            if want_ent:
+                ent = out[2]
+                if pre_ent is not None:
+                    ent_diff |= (ent != pre_ent[sl]).any()
+                if tau is None:                                             # masking with one chunk: the threshold of this pass
+                    tau = self._entropy_threshold(ent, completion_mask, rho)
+                out3, is_stats, ent_sum, dlp = ops.grpo_loss_ent_raw(
+                    lp, old[sl] if old is not None else None, ref[sl] if ref is not None else None, samp[sl] if tis else None, adv[sl],
+                    completion_mask[sl], ent, tau, self.beta, self.epsilon_low, self.epsilon_high, is_cap if tis else 2.0,
+                    want_grad=backward)
+                ent_acc += ent_sum
+            elif tis:
                 out3, is_stats, dlp = ops.grpo_loss_is_raw(lp, old[sl] if old is not None else None, ref[sl] if ref is not None else None,
                                                            samp[sl], adv[sl], completion_mask[sl], self.beta, self.epsilon_low,
                                                            self.epsilon_high, is_cap, want_grad=backward)
@@ -389,6 +444,12 @@ class DNALLMGRPOTrainer:
         if tis:
             for name, v in zip(("ratio_mean", "capped_frac", "logp_diff", "kl"), is_acc):
                 self._metrics[f"rollout_is/{name}"].append(v)
+        if want_ent:
+            if ent_diff is not None and bool(ent_diff):
+                raise RuntimeError("the entropy pre-pass and the loss pass disagree: the token mask would depend on the row chunking")
+            self._metrics["entropy"].append(ent_acc[0] / completion_mask.sum().clamp(min=1))
+            if masking:
+                self._metrics["entropy/threshold"].append(tau[0])
         return loss_acc[0]
 
     # ------------------------------------------------------------------ one optimizer step

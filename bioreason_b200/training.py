@@ -95,8 +95,9 @@ def plan_shared_prefix(G: int, P: int, L: int, kv_start: torch.Tensor, kv_end: t
 
 def policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_map, keep_last: int, *, save: bool = True,
                    lora="policy", targets: Optional[torch.Tensor] = None, dropout: bool = False, dropout_pass: Optional[int] = None,
-                   row_offset: int = 0, group_size: Optional[int] = None) -> "tuple[torch.Tensor, Optional[PolicyCtx]]":
-    """Returns (logps [B, keep_last] fp32, ctx).  lora: "policy" (adapters on), None (base weights = reference policy).
+                   row_offset: int = 0, group_size: Optional[int] = None, want_entropy: bool = False):
+    """Returns (logps [B, keep_last] fp32, ctx), or with want_entropy (logps, ctx, entropies [B, keep_last] fp32): the entropy of the
+    full-vocabulary softmax at every scored position (T = 1), from the same lm-head pass; the log-probs are the same bits.  lora: "policy" (adapters on), None (base weights = reference policy).
     targets: optional [B, keep_last] class ids scored at the last keep_last positions before the end (default: the realised next
     tokens input_ids[:, L-keep_last:]); entries < 0 are ignored (log-prob 0, no gradient) -- the SFT label mask.
     dropout: apply the LoRA dropout set by `model.set_lora_dropout` (no-op while it is off or with lora=None).  Row chunks of one pass
@@ -153,7 +154,10 @@ def policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_ma
         rows = plan.scored
     h_sel = ops.gather_rows(hn, rows)
     tgt = (input_ids[:, L - n:] if targets is None else targets.to(dev)).reshape(-1).to(torch.int32)
-    logp, lse = ops.lmhead_logprob(h_sel, W.lm_head, tgt)
+    if want_entropy:
+        logp, lse, ent = ops.lmhead_logprob(h_sel, W.lm_head, tgt, want_entropy=True)
+    else:
+        logp, lse = ops.lmhead_logprob(h_sel, W.lm_head, tgt)
     ctx = None
     if save:
         ctx = PolicyCtx()
@@ -164,6 +168,8 @@ def policy_forward(model, input_ids, attention_mask, dna_tokenized, batch_idx_ma
         ctx.use_lora = use_lora is not None
         ctx.drop = drop
         ctx.layout = plan
+    if want_entropy:
+        return logp.view(B, n), ctx, ent.view(B, n)
     return logp.view(B, n), ctx
 
 

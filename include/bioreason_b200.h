@@ -51,6 +51,19 @@ int br_grpo_loss_fwd_bwd(const float* lp, const float* old_lp, const float* ref_
 int br_grpo_loss_is_fwd_bwd(const float* lp, const float* old_lp, const float* ref_lp, const float* rollout_lp, const float* adv,
                             const int32_t* mask, int B, int C, float beta, float eps_low, float eps_high, float is_cap, float* out3,
                             float* is_stats, float* dlp, void* stream);
+/* The loss with high-entropy token selection (TRL's top_entropy_quantile, "Beyond the 80/20 Rule"): entropy [B, C] f32 per token
+ * (br_lmhead_logprob_entropy_fwd), tau [1] f32 on the device (br_entropy_threshold).  A token's clipped policy-gradient term and its
+ * gradient are kept only where mask && entropy >= *tau; the KL term, the per-row normalisation (sum of mask) and clip_ratio are
+ * unchanged.  rollout_lp optional: non-NULL adds the truncated importance weight of br_grpo_loss_is_fwd_bwd (is_stats, is_cap as
+ * there).  *tau = -inf reproduces br_grpo_loss_fwd_bwd / br_grpo_loss_is_fwd_bwd bit for bit.  ent_sum[1] = sum of mask * entropy.
+ * One launch. */
+int br_grpo_loss_ent_fwd_bwd(const float* lp, const float* old_lp, const float* ref_lp, const float* rollout_lp, const float* adv,
+                             const int32_t* mask, const float* entropy, const float* tau, int B, int C, float beta, float eps_low,
+                             float eps_high, float is_cap, float* out3, float* is_stats, float* ent_sum, float* dlp, void* stream);
+/* tau[0] = torch.quantile(entropy[mask != 0], level) (linear interpolation) bit for bit, on the device (no host sync): entropy [n]
+ * f32, mask [n] int32, level in [0, 1] (TRL: 1 - top_entropy_quantile).  Masked entries are not read as values.  No valid entry:
+ * tau = +inf.  -0 is read as +0.  One launch. */
+int br_entropy_threshold(const float* entropy, const int32_t* mask, int64_t n, float level, float* tau, void* stream);
 /* completion_mask[b, t] = t <= first_eos(b) (grpo_trainer.py:605-609); ids int64 [B, C] -> mask int32 */
 int br_eos_mask(const int64_t* completion_ids, int B, int C, int64_t eos_id, int32_t* mask, void* stream);
 
@@ -106,6 +119,13 @@ int br_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ldb, void* D
 int64_t br_lmhead_workspace_bytes(int M, int V);
 int br_lmhead_logprob_fwd(const void* H, int64_t ldh, const void* W, int64_t ldw, const int32_t* target,
                           int M, int V, int K, float scale, float* logp, float* lse, void* workspace, void* stream);
+/* br_lmhead_logprob_fwd plus the entropy of every row, target < 0 included:  entropy[m] = -sum_v p_v log p_v with
+ * p = softmax_v(scale*H[m].W[v]).  logp and lse are bit-identical to br_lmhead_logprob_fwd's.  Workspace:
+ * br_lmhead_entropy_workspace_bytes(M, V).  Two launches. */
+int64_t br_lmhead_entropy_workspace_bytes(int M, int V);
+int br_lmhead_logprob_entropy_fwd(const void* H, int64_t ldh, const void* W, int64_t ldw, const int32_t* target,
+                                  int M, int V, int K, float scale, float* logp, float* lse, float* entropy, void* workspace,
+                                  void* stream);
 /* dlogits[m, v] = gscale[m] * (onehot(target[m])[v] - softmax(H[m].W)[v]) as bf16 [M, ldd] (recomputed tiles) */
 int br_lmhead_dlogits(const void* H, int64_t ldh, const void* W, int64_t ldw, const int32_t* target,
                       const float* lse, const float* gscale, int M, int V, int K, float scale,
