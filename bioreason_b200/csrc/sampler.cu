@@ -8,18 +8,13 @@
 // cum <= 1 - p, always keep the best).  The draw is inverse-CDF over the kept tokens in ascending token id with a
 // caller-supplied uniform per (step, row): torch.multinomial's Philox consumption cannot be reproduced outside
 // torch, so parity is defined on supplied uniforms (SURVEY.md §7 "Sampling parity").
-// The *_proc entry points add HF's repetition penalty and min_new_tokens ahead of the warpers and min-p after top-p (see Proc below).
-#include "br_common.cuh"
+// The *_proc entry points add HF's repetition penalty and min_new_tokens ahead of the warpers and min-p after top-p (see Proc in sampler_common.cuh).
+#include "sampler_common.cuh"
 #include "../../include/bioreason_b200.h"
 
 namespace {
 
 constexpr int MAXC = 1024;
-
-__device__ __forceinline__ uint32_t fkey(float f) {
-    uint32_t u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
 
 // find bin b (descending scan) such that count(bins > b) < k <= count(bins >= b); returns b and updates k_rem
 __device__ int find_bin(const int* hist, int nbins, int& k_rem, int* s_tmp) {
@@ -81,29 +76,6 @@ __device__ void find_bin_asc(const int* hist, int k, int* out) {
     }
     if (lane == 0) { out[0] = found; out[1] = cnt; }
 }
-__device__ __forceinline__ float block_max(float v, float* s_red) {   // all threads get the maximum; s_red: 32 floats
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    if (lane == 0) s_red[warp] = v;
-    __syncthreads();
-    float m = lane < nw ? s_red[lane] : -INFINITY;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    __syncthreads();
-    return m;
-}
-// fixed-order block sum: thread 0 gets the total (the same bits on every call); s_red: 32 floats
-__device__ __forceinline__ float block_sum(float v, float* s_red) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-    v = br::warp_sum(v);
-    if (lane == 0) s_red[warp] = v;
-    __syncthreads();
-    float s = lane < nw ? s_red[lane] : 0.f;
-    s = br::warp_sum(s);
-    __syncthreads();
-    return s;
-}
 
 // Behaviour log-prob (the *_logp entry points): logp[r, step] = z[y] - logsumexp(z) over the raw fp32 logits of the row (T = 1, the
 // full vocabulary) -- the quantity br_lmhead_logprob_fwd gives the scoring passes.  Two-stage path: stage 1 writes each chunk's
@@ -117,28 +89,7 @@ __device__ __forceinline__ float block_sum(float v, float* s_red) {
 // and sets its overflow flag; stage 2 then selects on the logits row itself, so no tie HF keeps is lost.
 constexpr int CHUNK = 4096, CAND_CAP = 64;
 
-// Processed path (the *_proc entry points, PROC = true): HF's RepetitionPenalty -> MinNewTokens logits processors ahead of temperature /
-// top-k / top-p, and MinP after top-p.  Every kernel that reads a logit of the row applies proc_logit to it (stage 1 to the 16 values it
-// holds in registers, stage 2 and the single-stage sampler wherever they select on the row itself), so the candidates carry processed
-// values.  The log-prob stays on the raw row.  presence[r] is a bitmap of the tokens row r has emitted (bit j of word j / 32); the
-// sampler sets the emitted token's bit after the draw, one writer per row.
-struct Proc {
-    uint32_t* presence;           // [R, ceil(V / 32)], or nullptr: no penalty and no update
-    float theta;                  // repetition penalty
-    float min_p;                  // 0: off
-    int min_new;                  // EOS gets -inf while *step < min_new
-    long long eos;                // < 0: no EOS
-    const int* step;              // nullptr: step 0
-};
-
-// HF RepetitionPenaltyLogitsProcessor (z < 0 ? z * theta : z / theta, fp32, IEEE division) then MinNewTokensLengthLogitsProcessor
-__device__ __forceinline__ float proc_logit(float z, bool in_set, bool blocked, float theta) {
-    if (in_set) z = z < 0.f ? __fmul_rn(z, theta) : __fdiv_rn(z, theta);
-    return blocked ? -INFINITY : z;
-}
-__device__ __forceinline__ bool proc_in_set(const uint32_t* pres, int id) {
-    return pres != nullptr && ((__ldcg(pres + (id >> 5)) >> (id & 31)) & 1u);
-}
+// Processed path (the *_proc entry points, PROC = true): Proc and proc_logit in sampler_common.cuh.
 
 template <bool LOGP, bool PROC>
 __global__ void __launch_bounds__(256, 1) sampler_partial_kernel(const float* __restrict__ logits, long long ld, int V, int top_k,
@@ -713,17 +664,6 @@ int br_sample_next_2stage_logp(const float* logits, int64_t ld, int R, int V, fl
     BR_CHECK_ARG(logp, "sample_next_2stage_logp: no logp buffer");
     return sample_2stage<false>(logits, ld, R, V, temperature, top_k, top_p, do_sample, uniforms, step, max_steps, eos_id, pad_id, finished, tokens,
                                 next_ids, logp, workspace, stream);
-}
-
-// the processed entry points' arguments as the kernels take them; refuses what HF's processors refuse
-static int proc_args(const br_sample_proc* proc, int64_t eos_id, const int32_t* step, const char* what, Proc* out) {
-    BR_CHECK_ARG(proc, "%s: no br_sample_proc", what);
-    BR_CHECK_ARG(proc->repetition_penalty > 0.f, "%s: repetition_penalty must be > 0", what);
-    BR_CHECK_ARG(proc->min_p >= 0.f && proc->min_p <= 1.f, "%s: min_p must be in [0, 1]", what);
-    BR_CHECK_ARG(proc->min_new_tokens >= 0, "%s: min_new_tokens must be >= 0", what);
-    BR_CHECK_ARG(proc->repetition_penalty == 1.f || proc->presence, "%s: repetition_penalty != 1 needs a presence bitmap", what);
-    *out = Proc{proc->presence, proc->repetition_penalty, proc->min_p, proc->min_new_tokens, (long long)eos_id, step};
-    return BR_OK;
 }
 
 int br_sample_next_proc(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, int do_sample,

@@ -60,6 +60,10 @@ def _unbuilt_generation_args(kwargs, gc):
     return sorted(bad)
 
 
+# sampled rollouts with top_k above this (the top-k samplers' kept-set cap), or top_k = 0, use ops.sample_next_full
+FULL_VOCAB_TOP_K = 1024
+
+
 @dataclass
 class SamplingParams:
     max_new_tokens: int = 20
@@ -131,8 +135,11 @@ class SamplingParams:
         do_sample = bool(pick("do_sample", False))
         if n > 1 and not do_sample:
             raise ValueError(f"generate(): greedy decoding does not support num_return_sequences = {n} (as in HF); pass do_sample=True")
+        top_k = int(pick("top_k", 50) or 0)
+        if top_k < 0:
+            raise ValueError(f"generate(): top_k must be >= 0 (0: top-k off), got {top_k}")
         return cls(max_new_tokens=int(max_new if max_new is not None else 20), do_sample=do_sample,
-                   temperature=float(pick("temperature", 1.0)), top_k=int(pick("top_k", 50) or 0), top_p=float(pick("top_p", 1.0)),
+                   temperature=float(pick("temperature", 1.0)), top_k=top_k, top_p=float(pick("top_p", 1.0)),
                    eos_token_id=eos, pad_token_id=pad, repetition_penalty=theta, min_p=min_p, min_new_tokens=m, num_return_sequences=n)
 
 
@@ -312,6 +319,8 @@ class RolloutEngine:
         rep_pen = params.repetition_penalty
         min_p = params.min_p if params.do_sample else 0.0                   # HF applies min-p only when sampling
         min_new = params.min_new_tokens
+        # top_k = 0 (off) or above the 1024-value cap of the top-k samplers: the full-vocabulary sampler
+        full_vocab = params.do_sample and (params.top_k == 0 or params.top_k > FULL_VOCAB_TOP_K)
         key = (B, G, tuple(plen), C, n_shared, max_pages, n_pages, params.do_sample, params.temperature, params.top_k, params.top_p,
                params.eos_token_id, params.pad_token_id, id(Wd), bool(use_graph), bool(return_logprobs), rep_pen, min_p, min_new)
         St = self._cached.get(key)
@@ -371,7 +380,8 @@ class RolloutEngine:
             St.ssq_a = torch.zeros(n_part_, 32, device=dev, dtype=torch.float32)    # sum x^2 of the residual stream entering attention
             St.ssq_b = torch.zeros(n_part_, 32, device=dev, dtype=torch.float32)    # ... entering the MLP (see br_skinny_gemm)
             St.ssq_e = torch.zeros(1, 32, device=dev, dtype=torch.float32)          # ... of the embedding row (first layer)
-            St.samp_ws = ops.sample_workspace(R, cfg.vocab_size, dev, logp=return_logprobs)
+            St.samp_ws = (ops.sample_full_workspace(R, cfg.vocab_size, dev) if full_vocab
+                          else ops.sample_workspace(R, cfg.vocab_size, dev, logp=return_logprobs))
             # emitted-token bitmap of the repetition penalty (HF with inputs_embeds: only generated tokens count, not the prompt)
             St.presence = ops.presence_bitmap(R, cfg.vocab_size, dev) if rep_pen != 1.0 else None
             St.graph = None
@@ -394,6 +404,12 @@ class RolloutEngine:
         n_part = ((d + 127) // 128) * 4
 
         def sample(logits):
+            if full_vocab:
+                ops.sample_next_full(logits, workspace=samp_ws, temperature=params.temperature, top_k=params.top_k, top_p=params.top_p,
+                                     uniforms=uniforms, step=step, max_steps=C, eos_id=eos,
+                                     pad_id=params.pad_token_id if params.pad_token_id is not None else 0, finished=finished, tokens=tokens,
+                                     next_ids=next_ids, **samp_kw)
+                return
             ops.sample_next(logits, workspace=samp_ws, temperature=params.temperature, top_k=params.top_k, top_p=params.top_p, do_sample=params.do_sample,
                             uniforms=uniforms if params.do_sample else None, step=step, max_steps=C, eos_id=eos,
                             pad_id=params.pad_token_id if params.pad_token_id is not None else 0, finished=finished, tokens=tokens,

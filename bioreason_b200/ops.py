@@ -538,6 +538,40 @@ def _sample_next_proc(logits, R, V, temperature, top_k, top_p, do_sample, unifor
                                     ptr(logp, "float*"), proc, _stream()), "sample_next_proc")
 
 
+def sample_full_workspace(R, V, device):
+    """Workspace of sample_next_full (no initialisation needed)."""
+    return torch.empty(lib().br_sample_full_workspace_bytes(R, V), device=device, dtype=torch.uint8)
+
+
+def sample_next_full(logits, *, temperature=1.0, top_k=0, top_p=1.0, uniforms=None, step=None, max_steps=1, eos_id=-1, pad_id=0,
+                     finished=None, tokens=None, next_ids=None, workspace=None, logp=None, repetition_penalty=1.0, min_p=0.0,
+                     min_new_tokens=0, presence=None):
+    """Sample from the full vocabulary (br_sample_next_full): any top_k >= 0 (0: top-k off), no cap on the kept set.  The keyword
+    arguments mean what they mean in sample_next; workspace: sample_full_workspace(R, V, device)."""
+    R, V = logits.shape
+    assert logits.dtype == torch.float32
+    _need_cuda(logits, logp, presence)
+    assert workspace is not None and workspace.numel() >= lib().br_sample_full_workspace_bytes(R, V), \
+        "sample_next_full needs sample_full_workspace(R, V, device)"
+    if logp is not None:
+        assert logp.dtype == torch.float32 and logp.is_contiguous() and logp.shape == (R, max_steps), (logp.shape, R, max_steps)
+    proc = ffi.NULL
+    if repetition_penalty != 1.0 or min_p != 0.0 or min_new_tokens != 0:
+        if presence is not None:
+            assert presence.dtype == torch.int32 and presence.is_contiguous() and presence.shape == (R, (V + 31) // 32), \
+                ("presence must be int32 [R, ceil(V / 32)] contiguous", tuple(presence.shape), R, V)
+        proc = ffi.new("br_sample_proc*")
+        proc.repetition_penalty = float(repetition_penalty)
+        proc.min_p = float(min_p)
+        proc.min_new_tokens = int(min_new_tokens)
+        proc.presence = ptr(presence, "uint32_t*")
+    check(lib().br_sample_next_full(ptr(logits, "float*"), _row_major_2d(logits), R, V, float(temperature), int(top_k), float(top_p),
+                                    ptr(uniforms, "float*"), ptr(step, "int32_t*"), int(max_steps), int(eos_id), int(pad_id),
+                                    ptr(finished, "int32_t*"), ptr(tokens, "int64_t*"), ptr(next_ids, "int64_t*"), ptr(logp, "float*"),
+                                    proc, ptr(workspace), _stream()), "sample_next_full")
+    LAUNCHES[0] += (3 if 1 <= top_k < V else 0) + (3 if top_p < 1.0 else 0) + 1      # stats, the cuts' radix passes, draw
+
+
 def decode_advance(step, cur_len):
     check(lib().br_decode_advance(ptr(step, "int32_t*"), ptr(cur_len, "int32_t*"), cur_len.numel(), _stream()), "decode_advance")
 

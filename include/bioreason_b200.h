@@ -259,6 +259,21 @@ int br_sample_next_2stage_proc(const float* logits, int64_t ld, int R, int V, fl
                                const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id,
                                int32_t* finished, int64_t* tokens, int64_t* next_ids, float* logp, const br_sample_proc* proc,
                                void* workspace, void* stream);
+/* Full-vocabulary sampler: the draw above without the 1024-value cap, for any top_k >= 0 (0: top-k off).  z' is z after the
+ * processors of proc (NULL: none; min_p, repetition_penalty and min_new_tokens as above).  top_k >= 1 is clamped to V and keeps every
+ * value >= the k-th, ties included, with no cap; top-p orders the kept tokens by value desc, id asc, drops from the end while the
+ * cumulative probability at T is <= 1 - p (always keeping the first; among equal values the higher ids go first); min-p then drops
+ * exp((z'_j - z'_max) / T) < min_p; the draw is the inverse CDF over the kept tokens in ascending id.  Weights are
+ * exp((z' - max) / T), computed in fp64 and held as 64-bit fixed point (2^-40): the cuts and the draw are exact integer arithmetic on them.  logp (NULL: none)
+ * as in the *_logp entry points, bit-equal to br_sample_next_2stage_logp's for the same token.  A row with no finite z' draws pad_id.
+ * Refused: T <= 0, top_p <= 0, top_k < 0, no uniforms, V >= 2^23, and what the processed entry points refuse.  workspace:
+ * br_sample_full_workspace_bytes(R, V), no initialisation needed (the first kernel resets it).  Up to 8 kernels, chained with PDL; the
+ * sequence depends on (top_k, top_p) only, so a captured graph replays it. */
+int64_t br_sample_full_workspace_bytes(int R, int V);
+int br_sample_next_full(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p,
+                        const float* uniforms, const int32_t* step, int max_steps, int64_t eos_id, int64_t pad_id,
+                        int32_t* finished, int64_t* tokens, int64_t* next_ids, float* logp, const br_sample_proc* proc,
+                        void* workspace, void* stream);
 int br_decode_advance(int32_t* step, int32_t* cur_len, int R, void* stream);
 
 /* Decode attention, one launch per layer per step: per-head q/k RMSNorm + RoPE at cur_len[r], K/V append to the row's page,
