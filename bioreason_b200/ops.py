@@ -103,6 +103,78 @@ def grpo_loss_ent_raw(lp, old_lp, ref_lp, rollout_lp, adv, mask, entropy, tau, b
     return out3, stats, ent_sum, dlp
 
 
+def grpo_objective_raw(lp, old_lp, ref_lp, adv, mask, beta, eps_low, eps_high, *, norm_rows=0, norm=None, sequence_level=False,
+                       delta=None, rollout_lp=None, is_cap=2.0, entropy=None, tau=None, want_grad=True):
+    """The GRPO objectives of later TRL releases (br_grpo_objective_fwd_bwd): token or sequence-level (GSPO) ratios, two-sided clipping
+    with delta (None: off), optional truncated IS (rollout_lp) and entropy selection (entropy, tau).  Aggregation: norm_rows = B of the
+    whole local batch gives "grpo" (row means / B); otherwise norm, a device fp32 [1], divides the token sum (bnpo, dr_grpo, dapo).
+    Returns (out7, is_sums or None, ent_sum or None, dlp); out7 = [loss, sum of row-mean kl, clip, low, high, region, tokens] are
+    sums over this call's rows, so row chunks add up; is_sums are the masked sums behind grpo_loss_is_raw's means."""
+    _need_cuda(lp, adv, mask, norm, rollout_lp, entropy, tau)
+    B, C = lp.shape
+    assert (norm_rows > 0) != (norm is not None), "give norm_rows (grpo) or norm (bnpo / dr_grpo / dapo)"
+    lp = lp.float().contiguous()
+    old_lp = None if old_lp is None else old_lp.float().contiguous()
+    ref_lp = None if ref_lp is None else ref_lp.float().contiguous()
+    adv = adv.float().contiguous()
+    mask = mask.to(torch.int32).contiguous()
+    opt = ffi.new("br_grpo_objective*")
+    opt.sequence_level = 1 if sequence_level else 0
+    opt.delta = float("inf") if delta is None else float(delta)
+    opt.norm_rows = int(norm_rows)
+    if norm is not None:
+        norm = norm.float().reshape(1).contiguous()
+        opt.norm = ptr(norm, "float*")
+    is_sums = ent_sum = None
+    if rollout_lp is not None:
+        rollout_lp = rollout_lp.float().contiguous()
+        assert rollout_lp.shape == (B, C), (rollout_lp.shape, lp.shape)
+        is_sums = torch.empty(4, device=lp.device, dtype=torch.float32)
+        opt.rollout_lp, opt.is_cap, opt.is_sums = ptr(rollout_lp, "float*"), float(is_cap), ptr(is_sums, "float*")
+    if entropy is not None:
+        entropy = entropy.float().contiguous()
+        assert entropy.shape == (B, C) and tau is not None and tau.dtype == torch.float32 and tau.numel() == 1, (entropy.shape, lp.shape)
+        ent_sum = torch.empty(1, device=lp.device, dtype=torch.float32)
+        opt.entropy, opt.tau, opt.ent_sum = ptr(entropy, "float*"), ptr(tau, "float*"), ptr(ent_sum, "float*")
+    out7 = torch.empty(7, device=lp.device, dtype=torch.float32)
+    dlp = torch.empty_like(lp) if want_grad else None
+    check(lib().br_grpo_objective_fwd_bwd(ptr(lp, "float*"), ptr(old_lp, "float*"), ptr(ref_lp, "float*"), ptr(adv, "float*"),
+                                          ptr(mask, "int32_t*"), B, C, float(beta), float(eps_low), float(eps_high), opt,
+                                          ptr(out7, "float*"), ptr(dlp, "float*"), _stream()), "grpo_objective")
+    return out7, is_sums, ent_sum, dlp
+
+
+SCALE_REWARDS = {"group": 0, "batch": 1, "none": 2}
+
+
+def grpo_advantages_scaled(rewards_per_func: torch.Tensor, num_generations: int, scale_rewards: str = "group"):
+    """TRL's scale_rewards: (r - group mean) / (std + 1e-4) with the group std ("group", grpo_advantages' bits) or the std of all rows
+    ("batch"), or r - group mean ("none"); unbiased stds.  Returns (advantages, std_used [rows], zero_std [rows] int32); in "none"
+    mode std_used is the group std."""
+    _need_cuda(rewards_per_func)
+    r = rewards_per_func.float().contiguous()
+    rows, nf = r.shape
+    adv = torch.empty(rows, device=r.device, dtype=torch.float32)
+    sd = torch.empty_like(adv)
+    zero = torch.empty(rows, device=r.device, dtype=torch.int32)
+    check(lib().br_grpo_advantages_scaled(ptr(r, "float*"), rows, nf, num_generations, SCALE_REWARDS[scale_rewards], ptr(adv, "float*"),
+                                          ptr(sd, "float*"), ptr(zero, "int32_t*"), _stream()), "grpo_advantages_scaled")
+    return adv, sd, zero
+
+
+def eos_mask_truncated(completion_ids: torch.Tensor, eos_id: int):
+    """eos_mask with the rows that hold no EOS zeroed (mask_truncated_completions); returns (mask int32 [B, C], lengths int32 [B]), the
+    lengths counted before the zeroing."""
+    _need_cuda(completion_ids)
+    ids = completion_ids.to(torch.int64).contiguous()
+    B, C = ids.shape
+    m = torch.empty(B, C, device=ids.device, dtype=torch.int32)
+    n = torch.empty(B, device=ids.device, dtype=torch.int32)
+    check(lib().br_eos_mask_truncated(ptr(ids, "int64_t*"), B, C, int(eos_id), ptr(m, "int32_t*"), ptr(n, "int32_t*"), _stream()),
+          "eos_mask_truncated")
+    return m, n
+
+
 def entropy_threshold(entropy: torch.Tensor, mask: torch.Tensor, level: float) -> torch.Tensor:
     """fp32 [1] on the device: torch.quantile(entropy[mask != 0].float(), level) bit for bit (+inf when no entry is valid), without a
     host sync.  TRL's top_entropy_quantile rho takes level = 1 - rho."""

@@ -6,6 +6,7 @@ accepted and ignored exactly as the reference trainer ignores them.
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass, field
 from typing import Optional, Union
 
@@ -81,8 +82,29 @@ class DNALLMGRPOConfig:
     top_entropy_quantile: float = 1.0     # keep the policy-gradient term on the top rho fraction of completion tokens by entropy, over
                                           # all ranks per loss call (TRL; "Beyond the 80/20 Rule"); 1.0: off
     log_entropy: bool = False             # log the policy's mean token entropy (`entropy`) without masking
+    # the objectives of later TRL releases (DESIGN.md §3); the defaults are the reference's objective
+    loss_type: str = "grpo"               # "grpo": per-row token means, then the mean over rows; "bnpo": token mean over the local batch;
+                                          # "dr_grpo": token sum / (rows * max_completion_length); "dapo": token sum / (N / world), N the
+                                          # completion tokens of the micro-step over all ranks (TRL's num_items_in_batch)
+    importance_sampling_level: str = "token"   # "token"; "sequence": one ratio per row, exp(masked mean of lp - old) (GSPO)
+    delta: Optional[float] = None         # > 0: coef_1 <- min(coef_1, delta), two-sided clipping (INTELLECT-2); None: off
+    scale_rewards: str = "group"          # advantage divisor: "group" std, "batch" std, or "none"; True / False mean "group" / "none"
+    mask_truncated_completions: bool = False   # completions without EOS carry no loss (DAPO); not with suppress_eos
 
     def __post_init__(self):
+        if isinstance(self.scale_rewards, bool) or str(self.scale_rewards).lower() in ("true", "false"):
+            self.scale_rewards = "group" if str(self.scale_rewards).lower() == "true" else "none"
+        if self.scale_rewards not in ("group", "batch", "none"):
+            raise ValueError(f"scale_rewards must be 'group', 'batch' or 'none' (or a bool), got {self.scale_rewards!r}")
+        if self.loss_type not in ("grpo", "bnpo", "dr_grpo", "dapo"):
+            raise ValueError(f"loss_type must be 'grpo', 'bnpo', 'dr_grpo' or 'dapo', got {self.loss_type!r}")
+        if self.importance_sampling_level not in ("token", "sequence"):
+            raise ValueError(f"importance_sampling_level must be 'token' or 'sequence', got {self.importance_sampling_level!r}")
+        if self.delta is not None and not (isinstance(self.delta, (int, float)) and not isinstance(self.delta, bool)
+                                           and math.isfinite(self.delta) and self.delta > 0):
+            raise ValueError(f"delta must be None or a finite value > 0, got {self.delta!r}")
+        if self.mask_truncated_completions and self.suppress_eos:
+            raise ValueError("mask_truncated_completions with suppress_eos masks every completion: there would be nothing to train on")
         if not (0.0 <= self.top_entropy_quantile <= 1.0):
             raise ValueError(f"top_entropy_quantile must lie in [0, 1] (1.0: off), got {self.top_entropy_quantile}")
         if not (self.rollout_is_cap > 0):

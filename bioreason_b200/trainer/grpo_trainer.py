@@ -269,7 +269,16 @@ class DNALLMGRPOTrainer:
         if self.generation_kwargs.get("return_logprobs"):
             completion_ids, sampling_lp = completion_ids
         self.timings["rollout"] += time.perf_counter() - t0
-        completion_mask = ops.eos_mask(completion_ids, self.eos_token_id if not self.args.suppress_eos else -1)      # :605-609
+        eos = self.eos_token_id if not self.args.suppress_eos else -1
+        lengths = None
+        if getattr(self.args, "mask_truncated_completions", False):
+            # TRL: rows without EOS carry no loss and are masked out of the scoring passes too; rewards and completion_length see the
+            # completions as they were generated
+            completion_mask, lengths = ops.eos_mask_truncated(completion_ids, eos)
+            reward_mask = (torch.arange(completion_ids.shape[1], device=dev)[None, :] < lengths[:, None]).to(torch.int32)
+        else:
+            completion_mask = ops.eos_mask(completion_ids, eos)                                                       # :605-609
+            reward_mask = completion_mask
         # text reward functions need the ids on the host: start the copy now (side stream, pinned), wait for it only after the
         # reference-policy forward has been queued -> decode + CPU rewards overlap that forward
         need_text = rewards_per_func is None and any(not rw.wants_token_protocol(f) for f in self.reward_funcs)
@@ -289,15 +298,22 @@ class DNALLMGRPOTrainer:
         if rewards_per_func is None:
             t_r = time.perf_counter()
             rewards_per_func = rw.score(self.reward_funcs, examples=pi.get("_examples"), prompts=pi.get("_prompts"), completion_ids=completion_ids,
-                                        completion_mask=completion_mask, prompt_ids=prompt_ids, processing_class=self.processing_class,
+                                        completion_mask=reward_mask, prompt_ids=prompt_ids, processing_class=self.processing_class,
                                         host_copy=host_copy, extra_columns=pi.get("reward_kwargs"))
             self.timings["reward_host"] += time.perf_counter() - t_r
         rewards_all = dp.gather_rewards(rewards_per_func)                                                              # C1, :679
-        adv_all, gmean, gstd = ops.grpo_advantages(rewards_all, self.num_generations, return_stats=True)               # :682-692
+        scale = getattr(self.args, "scale_rewards", "group")
+        if scale != "group":
+            adv_all, std_used, zero_std = ops.grpo_advantages_scaled(rewards_all, self.num_generations, scale)
+            reward_std = std_used.mean()
+            self._metrics["frac_reward_zero_std"].append(zero_std.float().mean())
+        else:
+            adv_all, gmean, gstd = ops.grpo_advantages(rewards_all, self.num_generations, return_stats=True)           # :682-692
+            reward_std = gstd.mean()
         advantages = dp.local_slice(adv_all, B)                                                                        # :695-699
-        self._metrics["completion_length"].append(completion_mask.sum(1).float().mean())
+        self._metrics["completion_length"].append((lengths if lengths is not None else completion_mask.sum(1)).float().mean())
         self._metrics["reward"].append(rewards_all.sum(1).mean())
-        self._metrics["reward_std"].append(gstd.mean())
+        self._metrics["reward_std"].append(reward_std)
         for i, f in enumerate(self.reward_funcs):
             self._metrics[f"rewards/{getattr(f, '__name__', 'reward_' + str(i))}"].append(rewards_all[:, i].mean())
         self.timings["score"] += time.perf_counter() - t0
@@ -306,7 +322,19 @@ class DNALLMGRPOTrainer:
                    local_group_size=gs)
         if sampling_lp is not None:
             out["sampling_per_token_logps"] = sampling_lp
+        if getattr(self.args, "loss_type", "grpo") == "dapo":
+            # buffered with the inputs, so the num_iterations > 1 passes over this batch reuse it
+            out["num_items_in_batch"] = self._num_items_in_batch(lengths if lengths is not None else completion_mask)
         return out
+
+    @staticmethod
+    def _num_items_in_batch(counts):
+        """TRL's num_items_in_batch: the completion tokens (EOS-masked, counted before mask_truncated_completions) of all ranks, a
+        device fp32 [1]; one scalar all-reduce, no host sync."""
+        n = counts.sum().float().reshape(1)
+        if _world()[1] > 1:
+            dist.all_reduce(n)
+        return n
 
     @staticmethod
     def _auto_micro_rows(model, B, L):
@@ -392,6 +420,25 @@ class DNALLMGRPOTrainer:
                     tau = self._entropy_threshold(pre_ent, completion_mask, rho)
                     ent_diff = torch.zeros((), dtype=torch.bool, device=ids.device)
                 self.timings["entropy_prepass"] += time.perf_counter() - t0
+        # the objectives of later TRL releases (loss_type, sequence-level ratios, delta) run on br_grpo_objective_fwd_bwd, whose outputs
+        # are sums over a chunk's rows; the defaults keep the calls above
+        loss_type = getattr(self.args, "loss_type", "grpo")
+        seq_level = getattr(self.args, "importance_sampling_level", "token") == "sequence"
+        delta = getattr(self.args, "delta", None)
+        objective = loss_type != "grpo" or seq_level or delta is not None
+        if objective:
+            obj_acc = torch.zeros(7, device=ids.device)
+            if loss_type == "grpo":
+                norm_kw = dict(norm_rows=B)
+            elif loss_type == "bnpo":
+                norm_kw = dict(norm=completion_mask.sum().float().clamp(min=1).reshape(1))
+            elif loss_type == "dr_grpo":
+                norm_kw = dict(norm=torch.full((1,), float(B * self.max_completion_length), device=ids.device))
+            else:                                                           # dapo: the gradient average over ranks makes it the global mean
+                n = inputs.get("num_items_in_batch")
+                if n is None:
+                    n = self._num_items_in_batch(completion_mask)
+                norm_kw = dict(norm=n.clamp(min=1) / _world()[1])
         for lo in range(0, B, mr):
             hi = min(B, lo + mr)
             sl = slice(lo, hi)
@@ -409,6 +456,18 @@ class DNALLMGRPOTrainer:
                     ent_diff |= (ent != pre_ent[sl]).any()
                 if tau is None:                                             # masking with one chunk: the threshold of this pass
                     tau = self._entropy_threshold(ent, completion_mask, rho)
+            if objective:
+                out7, is_stats, ent_sum, dlp = ops.grpo_objective_raw(
+                    lp, old[sl] if old is not None else None, ref[sl] if ref is not None else None, adv[sl], completion_mask[sl], self.beta,
+                    self.epsilon_low, self.epsilon_high, sequence_level=seq_level, delta=delta, rollout_lp=samp[sl] if tis else None,
+                    is_cap=is_cap if tis else 2.0, entropy=ent if want_ent else None, tau=tau if want_ent else None, want_grad=backward,
+                    **norm_kw)
+                obj_acc += out7
+                if tis:
+                    is_acc += is_stats
+                if want_ent:
+                    ent_acc += ent_sum
+            elif want_ent:
                 out3, is_stats, ent_sum, dlp = ops.grpo_loss_ent_raw(
                     lp, old[sl] if old is not None else None, ref[sl] if ref is not None else None, samp[sl] if tis else None, adv[sl],
                     completion_mask[sl], ent, tau, self.beta, self.epsilon_low, self.epsilon_high, is_cap if tis else 2.0,
@@ -421,10 +480,13 @@ class DNALLMGRPOTrainer:
             else:
                 out3, dlp = ops.grpo_loss_raw(lp, old[sl] if old is not None else None, ref[sl] if ref is not None else None, adv[sl],
                                               completion_mask[sl], self.beta, self.epsilon_low, self.epsilon_high, want_grad=backward)
-            w = (hi - lo) / B
-            loss_acc += out3 * w                                            # row-mean of row-means is separable over row chunks
-            if tis:
-                is_acc += is_stats * w                                      # token means, row-weighted across chunks like clip_ratio
+            if objective:
+                w = 1.0                                                     # sums: the chunks add up
+            else:
+                w = (hi - lo) / B
+                loss_acc += out3 * w                                        # row-mean of row-means is separable over row chunks
+                if tis:
+                    is_acc += is_stats * w                                  # token means, row-weighted across chunks like clip_ratio
             self.timings["policy_fwd"] += time.perf_counter() - t0
             if backward:
                 t0 = time.perf_counter()
@@ -437,6 +499,14 @@ class DNALLMGRPOTrainer:
                 with self._mark("policy_bwd"):
                     training.policy_backward(model, ctx, dlp * (w / ga), on_layer_done=hook)
                 self.timings["policy_bwd"] += time.perf_counter() - t0
+        if objective:
+            # token means exact across row chunks; kl keeps its row-mean definition
+            n_tok = obj_acc[6].clamp(min=1)
+            loss_acc = torch.stack([obj_acc[0], obj_acc[1] / B, obj_acc[2] / n_tok])
+            for name, v in zip(("low_mean", "high_mean", "region_mean"), obj_acc[3:6] / n_tok):
+                self._metrics[f"clip_ratio/{name}"].append(v)
+            if tis:
+                is_acc = is_acc / n_tok
         # clip_ratio is a ratio of sums; with row chunks it is weighted by rows (exact when chunks have equal mask counts)
         if self.beta > 0:
             self._metrics["kl"].append(loss_acc[1])

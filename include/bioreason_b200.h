@@ -67,6 +67,44 @@ int br_entropy_threshold(const float* entropy, const int32_t* mask, int64_t n, f
 /* completion_mask[b, t] = t <= first_eos(b) (grpo_trainer.py:605-609); ids int64 [B, C] -> mask int32 */
 int br_eos_mask(const int64_t* completion_ids, int B, int C, int64_t eos_id, int32_t* mask, void* stream);
 
+/* The GRPO objectives of later TRL releases (DESIGN.md §3).  Ratio: token level s = lp - o, or sequence level (GSPO) one
+ * s_b = sum_t m (lp - o) / max(|o_b|, 1) per row; c1 = exp(s), c2 = clamp(c1, 1 - eps_low, 1 + eps_high), then c1 <- min(c1, delta)
+ * (torch.clamp(max=delta)); per token l = -min(c1 A, c2 A) w k + beta k3, w the truncated importance weight of
+ * br_grpo_loss_is_fwd_bwd (rollout_lp non-NULL), k the entropy keep-mask of br_grpo_loss_ent_fwd_bwd (entropy non-NULL).
+ * Aggregation: norm_rows > 0 gives sum_b (sum_t m l / max(|o_b|, 1)) / norm_rows ("grpo"; norm_rows = the rows of the whole
+ * local batch, so row chunks add up); norm_rows == 0 gives sum m l / *norm (norm [1] f32 on the device: bnpo, dr_grpo, dapo).
+ * The outputs are sums, so row chunks add up without reweighting:
+ *   out7 = {loss, sum_b of the row-mean k3 (rows with |o_b| > 0), sum m [c1 A < c2 A], sum m [c1 < 1 - eps_low && A < 0],
+ *           sum m [c1 > 1 + eps_high && A > 0], sum m [either], sum m};
+ *   is_sums[4] = the masked sums of br_grpo_loss_is_fwd_bwd's is_stats; ent_sum[1] = sum m * entropy.
+ * With sequence_level = 0, delta = +inf and norm_rows = B, out7 / dlp carry br_grpo_loss*_fwd_bwd's bits.  One launch. */
+typedef struct br_grpo_objective {
+    int32_t sequence_level;       /* 0: per-token ratio; 1: one ratio per row */
+    float delta;                  /* > 0; +inf: off */
+    int32_t norm_rows;            /* > 0: "grpo" aggregation over that many rows; 0: divide by *norm */
+    const float* norm;            /* [1] f32, device */
+    const float* rollout_lp;      /* optional [B, C] f32 */
+    float is_cap;                 /* > 0 when rollout_lp is given */
+    float* is_sums;               /* [4], needed with rollout_lp */
+    const float* entropy;         /* optional [B, C] f32 */
+    const float* tau;             /* [1] f32, device, needed with entropy */
+    float* ent_sum;               /* [1], needed with entropy */
+} br_grpo_objective;
+int br_grpo_objective_fwd_bwd(const float* lp, const float* old_lp, const float* ref_lp, const float* adv, const int32_t* mask, int B,
+                              int C, float beta, float eps_low, float eps_high, const br_grpo_objective* opt, float* out7, float* dlp,
+                              void* stream);
+/* Advantages with TRL's scale_rewards: (r - group mean) / (std + 1e-4) with std the unbiased group std (GROUP: br_grpo_advantages'
+ * bits), or the unbiased std of all rows (BATCH), or r - group mean (NONE).  std_used [rows] = the std of the row (the group std in
+ * NONE mode), zero_std [rows] int32 = std_used <= 1e-8.  One launch (one CTA). */
+#define BR_SCALE_REWARDS_GROUP 0
+#define BR_SCALE_REWARDS_BATCH 1
+#define BR_SCALE_REWARDS_NONE 2
+int br_grpo_advantages_scaled(const float* rewards_per_func, int rows, int n_funcs, int G, int mode, float* advantages, float* std_used,
+                              int32_t* zero_std, void* stream);
+/* br_eos_mask with the rows that hold no EOS zeroed (mask_truncated_completions); lengths [B] int32 = each row's mask count before
+ * that zeroing (min(first EOS + 1, C)).  A row with an EOS gets br_eos_mask's mask. */
+int br_eos_mask_truncated(const int64_t* completion_ids, int B, int C, int64_t eos_id, int32_t* mask, int32_t* lengths, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Dense contractions on wgmma (replaces every nn.Linear / lm_head reached through
  * dna_llm.py:150-160,237-242; SURVEY.md §2.3 K1,K2,K5,K6,K7,K12)
