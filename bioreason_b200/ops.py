@@ -330,6 +330,27 @@ def rmsnorm(x, w, eps: float, out=None, want_rstd: bool = False):
     return (out, rstd) if want_rstd else out
 
 
+def seqcls_score(h, input_ids, pad_id, norm_w, eps: float, score_w, out=None, want_index: bool = False):
+    """Pooled score head of a sequence-classification reward model (br_seqcls_score): h bf16 [B*L, d], the last decoder layer's
+    output before the final norm; input_ids [B, L].  Per row, the rightmost column whose id != pad_id (None: the last column) is
+    final-normed with norm_w and scored against score_w [n_labels, d].  Returns fp32 [B, n_labels] (and the pooled index int32 [B]
+    with want_index).  out: optional fp32 [B, n_labels] destination with contiguous rows, e.g. a column of rewards_per_func."""
+    _need_cuda(h, input_ids, norm_w, score_w, out)
+    B, L = input_ids.shape
+    n_labels, d = score_w.shape
+    assert h.dtype == torch.bfloat16 and score_w.dtype == torch.bfloat16 and norm_w.dtype == torch.bfloat16
+    assert h.shape == (B * L, d) and norm_w.shape == (d,), (h.shape, norm_w.shape, B, L, d)
+    ids = input_ids.to(torch.int64).contiguous()
+    if out is None:
+        out = torch.empty(B, n_labels, device=h.device, dtype=torch.float32)
+    assert out.dtype == torch.float32 and out.shape == (B, n_labels) and out.stride(1) == 1, (out.dtype, out.shape, out.stride())
+    idx = torch.empty(B, device=h.device, dtype=torch.int32) if want_index else None
+    check(lib().br_seqcls_score(ptr(h), _row_major_2d(h), ptr(ids, "int64_t*"), B, L, -1 if pad_id is None else int(pad_id), ptr(norm_w),
+                                float(eps), ptr(score_w), _row_major_2d(score_w), n_labels, d, ptr(out, "float*"), out.stride(0),
+                                ptr(idx, "int32_t*"), _stream()), "seqcls_score")
+    return (out, idx) if want_index else out
+
+
 def layernorm(x, w, b, eps: float, out=None):
     _need_cuda(x, w, b)
     M, d = x.shape

@@ -102,7 +102,7 @@ class DecoderLayerW:
 class DecoderW:
     cfg: object
     embed: torch.Tensor            # [V, d] (tied lm_head)
-    lm_head: torch.Tensor          # [V, d]
+    lm_head: Optional[torch.Tensor]   # [V, d]; None for a sequence classifier (RewardModel), which has a score head instead
     final_norm: torch.Tensor
     layers: List[DecoderLayerW] = field(default_factory=list)
     lm_head_T: Optional[torch.Tensor] = None   # [d, V] for dH = dlogits @ W
@@ -115,15 +115,21 @@ class DecoderW:
             self.lm_head_T = self.lm_head.t().contiguous()
 
 
-def pack_decoder(model, device="cuda") -> DecoderW:
-    """Fuse a HF Qwen3ForCausalLM's weights into kernel layout (bf16, on `device`) and re-point its parameters."""
+def pack_decoder(model, device="cuda", lm_head: bool = True) -> DecoderW:
+    """Fuse a HF Qwen3ForCausalLM's weights into kernel layout (bf16, on `device`) and re-point its parameters.
+
+    lm_head=False packs the trunk of a frozen forward-only model without an lm_head (Qwen3ForSequenceClassification): W.lm_head is
+    None, and the container's gate / up parameters move to the host, so the kernel copy is the only device copy of them (about
+    2 bytes per parameter resident)."""
     cfg = model.config
     d = cfg.hidden_size
     bf = torch.bfloat16
     emb_p = model.model.embed_tokens.weight
     embed = torch.empty(emb_p.shape, device=device, dtype=bf)
     _repoint(emb_p, embed)
-    if cfg.tie_word_embeddings:
+    if not lm_head:
+        lm_head = None
+    elif cfg.tie_word_embeddings:
         model.lm_head.weight = model.model.embed_tokens.weight
         lm_head = embed
     else:
@@ -139,7 +145,9 @@ def pack_decoder(model, device="cuda") -> DecoderW:
             for t, rows in zip(f.targets, f.rows(cfg)):
                 p = getattr(getattr(layer, f.parent), t).weight
                 if f.blocked:
-                    p.data = p.data.to(device=device, dtype=bf)             # own storage: _copy_blocked fills the kernel copy
+                    # own storage: _copy_blocked fills the kernel copy.  Nothing re-derives a forward-only trunk's copy (lm_head=False), so
+                    # its container keeps that storage on the host
+                    p.data = p.data.to(device=device, dtype=bf) if lm_head is not None else p.data.to("cpu")
                 else:
                     _repoint(p, w[rows])
         small = {}

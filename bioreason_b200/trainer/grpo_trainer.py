@@ -96,7 +96,6 @@ class DNALLMGRPOTrainer:
         assert not isinstance(model, str), "model must be a DNALLMModel instance"             # grpo_trainer.py:241
         self.model, self.args = model, args or DNALLMGRPOConfig()
         a = self.args
-        self.reward_funcs = list(reward_funcs) if isinstance(reward_funcs, (list, tuple)) else [reward_funcs]
         self.dna_module, self.processing_class = dna_module, processing_class
         self.train_dataset, self.eval_dataset = train_dataset, eval_dataset
         self.num_generations, self.max_completion_length = a.num_generations, a.max_completion_length
@@ -113,6 +112,9 @@ class DNALLMGRPOTrainer:
         if getattr(a, "share_prompt_prefix", False) and a.apply_lora_dropout:
             raise ValueError("share_prompt_prefix cannot be combined with apply_lora_dropout: the dropout masks differ between the G copies "
                              "of a prompt, so the prompt cannot be computed once")
+        # reward models (paths or sequence classifiers) are packed next to the policy now, so an unsupported one fails before any step
+        self.reward_funcs, self.reward_processing_classes = rw.resolve_reward_funcs(reward_funcs, reward_processing_classes,
+                                                                                    a.model_init_kwargs, model._dec.embed.device)
         if model._lora is None:
             model.enable_lora(r=a.lora_r, alpha=a.lora_alpha, seed=a.seed)
         # each rank quantizes its own (identical) merged weights; the quantizer is deterministic, so the ranks agree
@@ -299,7 +301,8 @@ class DNALLMGRPOTrainer:
             t_r = time.perf_counter()
             rewards_per_func = rw.score(self.reward_funcs, examples=pi.get("_examples"), prompts=pi.get("_prompts"), completion_ids=completion_ids,
                                         completion_mask=reward_mask, prompt_ids=prompt_ids, processing_class=self.processing_class,
-                                        host_copy=host_copy, extra_columns=pi.get("reward_kwargs"))
+                                        host_copy=host_copy, extra_columns=pi.get("reward_kwargs"),
+                                        reward_processing_classes=self.reward_processing_classes)
             self.timings["reward_host"] += time.perf_counter() - t_r
         rewards_all = dp.gather_rewards(rewards_per_func)                                                              # C1, :679
         scale = getattr(self.args, "scale_rewards", "group")
@@ -315,7 +318,7 @@ class DNALLMGRPOTrainer:
         self._metrics["reward"].append(rewards_all.sum(1).mean())
         self._metrics["reward_std"].append(reward_std)
         for i, f in enumerate(self.reward_funcs):
-            self._metrics[f"rewards/{getattr(f, '__name__', 'reward_' + str(i))}"].append(rewards_all[:, i].mean())
+            self._metrics[f"rewards/{rw.reward_func_name(f, i)}"].append(rewards_all[:, i].mean())
         self.timings["score"] += time.perf_counter() - t0
         out = dict(prompt_ids=prompt_ids, prompt_mask=prompt_mask, completion_ids=completion_ids, completion_mask=completion_mask,
                    old_per_token_logps=old_lp, ref_per_token_logps=ref_lp, advantages=advantages, multimodal_inputs=mm,

@@ -12,7 +12,12 @@ The reference decodes the completions with `processing_class.batch_decode(..., s
   for that event only, so decoding + the CPU reward functions overlap the reference-policy forward that is already
   queued on the compute stream (SURVEY.md §8f-2).
 
-Everything in this file is host logic (no kernels): it is covered by tests/test_rewards_cpu.py.
+A reward function may also be a sequence-classification model (a path or a `PreTrainedModel`, grpo_trainer.py:343-368), run as a
+`RewardModel` on the CUDA decoder: the texts are built and tokenized on the host as the reference does (:656-663) and the model writes
+its column of rewards_per_func on the device.
+
+Everything in this file is host logic (the reward model's device work is in reward_model.py): it is covered by
+tests/test_rewards_cpu.py and tests/test_reward_model_cpu.py.
 """
 from __future__ import annotations
 
@@ -20,6 +25,8 @@ import inspect
 from typing import Any, Callable, Dict, List, Optional, Sequence
 
 import torch
+
+from ..reward_model import RewardModel
 
 
 def is_conversational(example: Dict[str, Any]) -> bool:
@@ -80,6 +87,56 @@ def _side_stream(device):
     return _SIDE[key]
 
 
+def apply_chat_template(example: Dict[str, Any], tokenizer) -> Dict[str, str]:
+    """trl.data_utils.apply_chat_template restated for the "messages" key, the only one the reward-model texts use."""
+    return {"text": tokenizer.apply_chat_template(example["messages"], tokenize=False)}
+
+
+def reward_func_name(f, i: int) -> str:
+    """The metric suffix of reward function i (grpo_trainer.py:707-711): a model's last path component, else the function name."""
+    if isinstance(f, RewardModel):
+        return f.config._name_or_path.split("/")[-1]
+    return getattr(f, "__name__", f"reward_{i}")
+
+
+def resolve_reward_funcs(reward_funcs, reward_processing_classes, model_init_kwargs, device):
+    """grpo_trainer.py:341-370: paths load as AutoModelForSequenceClassification(num_labels=1), every model gets a tokenizer (its own
+    directory's by default, pad = eos when it has none, config.pad_token_id set to it) and is packed as a RewardModel on `device`.
+    Returns (reward_funcs, reward_processing_classes), one entry per function (None for callables)."""
+    funcs = list(reward_funcs) if isinstance(reward_funcs, (list, tuple)) else [reward_funcs]
+    if reward_processing_classes is None:
+        procs = [None] * len(funcs)
+    elif not isinstance(reward_processing_classes, list):
+        procs = [reward_processing_classes]
+    else:
+        if len(reward_processing_classes) != len(funcs):
+            raise ValueError("The number of reward processing classes must match the number of reward functions.")
+        procs = list(reward_processing_classes)
+    procs += [None] * (len(funcs) - len(procs))
+    from transformers import AutoModelForSequenceClassification, AutoTokenizer, PreTrainedModel
+    for i, f in enumerate(funcs):
+        if isinstance(f, str):
+            f = AutoModelForSequenceClassification.from_pretrained(f, num_labels=1, **(model_init_kwargs or {}))
+        if not isinstance(f, PreTrainedModel):
+            continue
+        proc = procs[i]
+        if proc is None:
+            proc = AutoTokenizer.from_pretrained(f.config._name_or_path)
+        if proc.pad_token_id is None:
+            proc.pad_token = proc.eos_token
+        # the pooled token is the rightmost one that is not the tokenizer's pad
+        f.config.pad_token_id = proc.pad_token_id
+        funcs[i], procs[i] = RewardModel(f, device), proc
+    return funcs, procs
+
+
+def model_reward_texts(tokenizer, prompts, completions, conversational: bool) -> List[str]:
+    """grpo_trainer.py:656-660: the prompt + completion text each row is scored on."""
+    if conversational:
+        return [apply_chat_template({"messages": p + c}, tokenizer)["text"] for p, c in zip(prompts, completions)]
+    return [p + c for p, c in zip(prompts, completions)]
+
+
 def decode_completions(processing_class, completion_ids_host: torch.Tensor, conversational: bool):
     """grpo_trainer.py:640-645."""
     if processing_class is None or not hasattr(processing_class, "batch_decode"):
@@ -94,8 +151,10 @@ def decode_completions(processing_class, completion_ids_host: torch.Tensor, conv
 
 def score(reward_funcs: Sequence[Callable], *, examples: Optional[Sequence[Dict[str, Any]]], prompts: Optional[List[Any]],
           completion_ids: torch.Tensor, completion_mask: torch.Tensor, prompt_ids: torch.Tensor, processing_class,
-          host_copy: Optional[AsyncHostCopy] = None, extra_columns: Optional[Dict[str, List[Any]]] = None) -> torch.Tensor:
-    """rewards_per_func [B, n_funcs] fp32 on completion_ids.device, reference protocol by default (see module docstring)."""
+          host_copy: Optional[AsyncHostCopy] = None, extra_columns: Optional[Dict[str, List[Any]]] = None,
+          reward_processing_classes: Optional[Sequence[Any]] = None) -> torch.Tensor:
+    """rewards_per_func [B, n_funcs] fp32 on completion_ids.device, reference protocol by default (see module docstring).
+    reward_processing_classes: the tokenizer of each RewardModel function (resolve_reward_funcs), None elsewhere."""
     B = completion_ids.shape[0]
     dev = completion_ids.device
     out = torch.zeros(B, len(reward_funcs), device=dev, dtype=torch.float32)
@@ -111,6 +170,20 @@ def score(reward_funcs: Sequence[Callable], *, examples: Optional[Sequence[Dict[
         if extra_columns:
             columns.update(extra_columns)
     for i, f in enumerate(reward_funcs):
+        if isinstance(f, RewardModel):
+            if any(not isinstance(p, (str, list)) for p in prompts):
+                raise ValueError("a reward model scores prompt + completion text: the batch needs its prompts (examples with a "
+                                 "'prompt' key, or a 'prompts' list next to a tokenised batch)")
+            tok = reward_processing_classes[i] if reward_processing_classes is not None else None
+            if tok is None:
+                raise ValueError(f"reward function {i} is a reward model and needs its reward processing class (tokenizer)")
+            texts = model_reward_texts(tok, prompts, completions, conv)
+            enc = tok(texts, return_tensors="pt", padding=True, padding_side="right", add_special_tokens=False)
+            if f.num_labels == 1:
+                f(enc["input_ids"], enc["attention_mask"], out=out[:, i:i + 1])
+            else:                                                   # the reference takes logits[:, 0]
+                out[:, i] = f(enc["input_ids"], enc["attention_mask"])[:, 0]
+            continue
         if i in text_funcs:
             vals = f(prompts=prompts, completions=completions, **columns)
         else:

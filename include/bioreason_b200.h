@@ -177,6 +177,14 @@ int br_lmhead_dlogits(const void* H, int64_t ldh, const void* W, int64_t ldw, co
 /* y = w * bf16(x * rsqrt(mean(x^2)+eps)); bf16 [M, d]; rstd [M] f32 optional (kept for the backward) */
 int br_rmsnorm(const void* x, int64_t ldx, const void* w, void* y, int64_t ldy, float* rstd, int M, int d, float eps, void* stream);
 int br_layernorm(const void* x, int64_t ldx, const void* w, const void* b, void* y, int64_t ldy, int M, int d, float eps, void* stream);
+/* Pooled score head of a sequence-classification reward model (HF GenericForSequenceClassification): h bf16 [B*L, ldh] is the last
+ * decoder layer's output BEFORE the final norm, input_ids int64 [B, L].  Per row: t = the rightmost column whose id != pad_id, over
+ * all L columns (0 when every column is pad; pad_id = -1: none, t = L - 1); y = bf16(norm_w * bf16(h[t] * rsqrt(mean(h[t]^2) + eps)))
+ * with an fp32 sum of squares; out[b * ldo + j] = float(bf16(sum_i y_i score_w[j, i])) with fp32 accumulation, j < n_labels.
+ * index (NULL: not written) int32 [B] receives t.  d % 8 == 0, d <= 10240.  One launch, one CTA per row, fixed-order reductions:
+ * the same bits on every launch. */
+int br_seqcls_score(const void* h, int64_t ldh, const int64_t* input_ids, int B, int L, int64_t pad_id, const void* norm_w, float eps,
+                    const void* score_w, int64_t ldw, int n_labels, int d, float* out, int64_t ldo, int32_t* index, void* stream);
 /* In place on the fused QKV activation [M, ld]: heads 0..n_q-1 are queries, the next n_k are keys.
  * mode 0 (Qwen3): per-head RMSNorm with q_norm_w / k_norm_w [head_dim] (NULL = skip) then rotate-half RoPE;
  * mode 1 (ESM/NT-v2): queries scaled by q_scale, then RoPE.  positions [M] int32 (explicit: the reference uses
