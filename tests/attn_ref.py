@@ -1,6 +1,7 @@
 """fp64 reference of the training attention (causal GQA, one key window [ks, ke) per row), its analytic backward, a per-element
 error bound for the bf16-in / fp32-accumulate kernels, and seeded input families in which the mask edges decide an O(1) share of
-the result.  Test infrastructure: torch only, runs on CPU or GPU; oracle/ is not involved.
+the result.  causal=False gives the bidirectional encoder attention (every query of a row sees the whole window; the rows past
+kv_end are pad queries and still get a result).  Test infrastructure: torch only, runs on CPU or GPU; oracle/ is not involved.
 
 Layouts: q, do [B, L, Hq, D]; k, v [B, L, Hkv, D]; lse [B, Hq, L].  The shared-prefix layout ([U * Lp prefix rows | U * G suffixes])
 is checked through its dense equivalent: expand_shared() builds the [U * G, Lp + Ls] rows, fold_shared() maps dense results back
@@ -29,15 +30,23 @@ FAR = 300.0                  # magnitude of the k / v rows outside the window in
 
 # one typical kernel bug each; attn_ref(variant=...) computes attention as a kernel carrying it would
 VARIANTS = ("diag_strict", "diag_plus_1", "ks_minus_1", "ke_included", "head_mod", "no_rescale")
+# the same for the bidirectional (causal=False) kernel; tail_tile_unmasked: the keys from ke to the end of the 64-key tile that holds
+# ke - 1 (the last tile the kernel loads) are left visible
+NONCAUSAL_VARIANTS = ("causal_applied", "ke_included", "ks_minus_1", "tail_tile_unmasked", "no_rescale")
 
 
-def visible(L, ks, ke, device, variant=None):
+def visible(L, ks, ke, device, variant=None, causal=True):
     """[L, L] bool: query i sees key j."""
     i = torch.arange(L, device=device)[:, None]
     j = torch.arange(L, device=device)[None, :]
     lo = ks - 1 if variant == "ks_minus_1" and ks > 0 else ks
     hi = ke + 1 if variant == "ke_included" and ke < L else ke
-    diag = (j < i) if variant == "diag_strict" else (j <= i + 1) if variant == "diag_plus_1" else (j <= i)
+    if variant == "tail_tile_unmasked":
+        hi = min(L, -(-ke // BN) * BN)
+    if causal:
+        diag = (j < i) if variant == "diag_strict" else (j <= i + 1) if variant == "diag_plus_1" else (j <= i)
+    else:
+        diag = (j <= i) if variant == "causal_applied" else torch.ones(L, L, dtype=torch.bool, device=device)
     return (j >= lo) & (j < hi) & diag
 
 
@@ -65,7 +74,7 @@ def _online_softmax_fwd(S, vis, vh, rescale):
     return o, lse
 
 
-def attn_ref(q, k, v, do, windows, *, scale=None, o_used=None, variant=None, bounds=True):
+def attn_ref(q, k, v, do, windows, *, scale=None, o_used=None, variant=None, bounds=True, causal=True):
     """Forward and analytic backward in float64 from the exact input values, plus the per-element bounds (see the module doc).
 
     windows: [(ks, ke)] per row.  o_used: the O the backward under test reads ([B, L, Hq, D]); it sets Edelta.  Without it Edelta
@@ -77,7 +86,8 @@ def attn_ref(q, k, v, do, windows, *, scale=None, o_used=None, variant=None, bou
     GQ = Hq // Hkv
     dev = q.device
     f64 = lambda t: t.to(torch.float64)
-    q, k, v, do = f64(q), f64(k), f64(v), f64(do)
+    q, k, v = f64(q), f64(k), f64(v)
+    do = torch.zeros_like(q) if do is None else f64(do)
     o_used = None if o_used is None else f64(o_used)
     scale = D ** -0.5 if scale is None else scale
     u, w = U_BF16, W_ACC
@@ -89,7 +99,7 @@ def attn_ref(q, k, v, do, windows, *, scale=None, o_used=None, variant=None, bou
     kv_of = (lambda h: h % Hkv) if variant == "head_mod" else (lambda h: h // GQ)
     for b in range(B):
         ks, ke = (int(x) for x in windows[b])
-        vis = visible(L, ks, ke, dev, variant)
+        vis = visible(L, ks, ke, dev, variant, causal)
         for hk in range(Hkv):
             heads = [h for h in range(Hq) if kv_of(h) == hk]
             if not heads:
@@ -169,7 +179,7 @@ def fold_shared(t, U, G, Lp, Ls, prefix="sum"):
 
 
 # ------------------------------------------------------------------------------------------------------------- input families
-def make_inputs(family, B, L, Hq, Hkv, windows, *, D=128, seed=0, device="cpu", group=None):
+def make_inputs(family, B, L, Hq, Hkv, windows, *, D=128, seed=0, device="cpu", group=None, causal=True):
     """Seeded bf16 q, k, v, do on `device` (drawn on the CPU, so every device sees the same values).
 
     random    : N(0, 0.7^2) q / k / v, N(0, 1) dO.
@@ -178,9 +188,12 @@ def make_inputs(family, B, L, Hq, Hkv, windows, *, D=128, seed=0, device="cpu", 
                 past it a larger, masked decoy (~17).
     first_key : every query shares a direction e per KV head; k at ks = e scaled to a score of ~12, so the maximum sits in the
                 first key tile and the later tiles must leave it alone.
+    window_decoy (for causal=False): every query shares a direction e per KV head as in first_key, the key at ke - 1 is e scaled to a
+                score of ~12 (the maximum sits in the last key tile, so every earlier tile must be rescaled), and every key outside
+                the window is +300 e: any key that leaks through the mask takes every query row.
     In decoy and first_key the k / v rows outside the window are +-300 (finite: a leaked key takes the whole row), and the rows at
     ks - 1 and ke (where they exist) are explicit decoys: 300 * sign of the query at ks (resp. ke), the first query that would
-    see them through an off-by-one.
+    see them through an off-by-one (with causal=False every query sees them: both use the query at ks).
     group=(G, Lp): rows b of one group b // G share positions [0, Lp) (the shared-prefix layout's dense equivalent)."""
     gen = torch.Generator().manual_seed(seed)
     GQ = Hq // Hkv
@@ -197,14 +210,14 @@ def make_inputs(family, B, L, Hq, Hkv, windows, *, D=128, seed=0, device="cpu", 
             qr = ch[None, :, None] * math.sqrt(D) * ud.repeat_interleave(GQ, 1)
             kr = 11.0 * ud
             kr[1:] += 17.0 * ud[:-1]
-        elif family == "first_key":
+        elif family in ("first_key", "window_decoy"):
             e = torch.randn(Hkv, D, generator=gen)
             e = e / e.norm(dim=-1, keepdim=True)
             t = 0.7 * math.sqrt(D)
             qr = torch.randn(L, Hq, D, generator=gen) * 0.7 + t * e.repeat_interleave(GQ, 0)[None]
             kr = torch.randn(L, Hkv, D, generator=gen) * 0.7
             if ks < ke:
-                kr[ks] = (12.0 / (scale * t)) * e
+                kr[ks if family == "first_key" else ke - 1] = (12.0 / (scale * t)) * e
         else:
             raise ValueError(family)
         vr = torch.randn(L, Hkv, D, generator=gen) * 0.7
@@ -213,7 +226,10 @@ def make_inputs(family, B, L, Hq, Hkv, windows, *, D=128, seed=0, device="cpu", 
         n_out = int(out.sum())
         kr[out] = FAR * torch.randn(n_out, Hkv, D, generator=gen).sign()
         vr[out] = FAR * torch.randn(n_out, Hkv, D, generator=gen).sign()
-        for jd, iq in ((ks - 1, ks), (ke, ke)):
+        if family == "window_decoy":
+            kr[out] = FAR * e
+            return qr, kr, vr
+        for jd, iq in ((ks - 1, ks), (ke, ke if causal else ks)):
             if 0 <= jd < L and iq < L:
                 kr[jd] = FAR * qr[iq, ::GQ].sign()
         return qr, kr, vr
